@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the NAM inference hot path on B200 (one JSON line, driver contract).
+"""bench.py -- throughput of the NAM inference hot path on H100 (one JSON line).
 
 Workload (BASELINE.json metric): wavenet_a1_standard.nam, batch 4096 independent 48 kHz streams per GPU,
 float32.  A "step" is ONE pass of the hot path over one batch of synthetic input: 4096 streams x
@@ -10,13 +10,17 @@ streams are independent, SURVEY.md 8e).
   value      Msamples/s, whole job, inputs/outputs resident in HBM, CUDA-event timed, max over ranks
   e2e        same metric through the public host API (nam_b200_process_f32 with pinned host buffers:
              H2D + kernel + D2H inside the timed region)
-  roofline   the fused kernel against the FP32 FMA pipe (self-measured FFMA2 peak) -- the binding roof
+  roofline   the fused kernel against the FP32 FMA pipe (self-measured FFMA peak) -- the binding roof
              for this path (DESIGN.md "Roofline") -- plus HBM / tensor fractions for context
   cpu_baseline  the CPU restatement (oracle/, "port") on all host cores, bounded sample
   --impl reference   times that CPU port as the reference arm (the reference itself cannot be built
              here: Eigen is an un-vendored submodule, see DESIGN.md)
 
-Nothing here reads /root/reference.
+  --dump-outputs DIR   after the timed steps, the outputs of the last one as DIR/*.npy (float32; a fixed sample
+             of the streams when all of them would exceed 32 MiB, shared by all ranks), so that two builds can be compared output for
+             output: with the same arguments the inputs are the same on every run
+
+Nothing here reads the reference's source tree.
 """
 from __future__ import annotations
 
@@ -60,7 +64,26 @@ def parse_args():
     ap.add_argument("--no-secondary", action="store_true", help="skip the quick batch-1/256, A2, LSTM, a2_max lines")
     ap.add_argument("--no-gather", action="store_true",
                     help="N > 1: skip the second timed pass that all-gathers every step's outputs over NCCL")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/*.npy (float32)")
     return ap.parse_args()
+
+
+DUMP_MAX_BYTES = 32 << 20
+
+
+def dump_outputs(out_dir: str, y: np.ndarray, name: str = "y", budget: int = DUMP_MAX_BYTES) -> None:
+    """y [streams, frames] -> out_dir/<name>.npy, all streams if they fit in `budget` bytes, else a fixed (seeded) sample
+    of whole streams, in stream order, with their indices in out_dir/<name>_streams.npy."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    y = np.asarray(y, dtype=np.float32)
+    keep = max(1, min(y.shape[0], budget // max(1, y.shape[1] * 4)))
+    if keep < y.shape[0]:
+        rows = np.sort(np.random.default_rng(0).choice(y.shape[0], size=keep, replace=False))
+        y = y[rows]
+        np.save(d / f"{name}_streams.npy", rows.astype(np.float64))
+    np.save(d / f"{name}.npy", np.ascontiguousarray(y))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -73,7 +96,8 @@ def load_peaks() -> dict:
             return d
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "_source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -230,7 +254,7 @@ def cpu_arms(nam: dict, fast_tanh: bool, frames: int, streams_per_thread: int) -
         if r is not None:
             out["reference"] = {"value": r[0], "seconds": r[1], "cores": cores, "streams": streams,
                                 "flags": f"g++ -Ofast -march={'x86-64-v4' if r[2] == 'fast512' else 'x86-64-v3'} "
-                                         "(tools/CMakeLists.txt:106), unmodified /root/reference/NAM sources, Eigen stand-in"}
+                                         "(tools/CMakeLists.txt:106), unmodified reference NAM sources, Eigen stand-in"}
     except Exception as exc:  # the reference build is optional on the box
         out["reference_error"] = str(exc)[:200]
     kind = "reference" if out.get("reference", {}).get("value", 0.0) > v else "port"
@@ -271,6 +295,8 @@ def run_reference(args) -> None:
         pool.process(x, y, CPU_BLOCK, cores)
     dt = time.perf_counter() - t0
     pool.close()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, y)
     value = streams * args.frames * args.steps / dt / 1e6
     port_value = value
     sample = (f"{streams} of {args.batch} streams x {args.frames} frames per step in {CPU_BLOCK}-frame process() calls "
@@ -403,6 +429,9 @@ def run_b200(args) -> None:
             step_device()
             ev[i + 1].record(stream)
         barrier()
+    if args.dump_outputs:
+        # every rank writes its own streams; the ranks share one DUMP_MAX_BYTES budget
+        dump_outputs(args.dump_outputs, y_dev.cpu().numpy(), "y" if world == 1 else f"y_rank{rank}", DUMP_MAX_BYTES // world)
     total_ms = ev[0].elapsed_time(ev[-1])
     step_ms = [ev[i].elapsed_time(ev[i + 1]) for i in range(args.steps)]
     launches = model.launch_count() - launches0
@@ -441,7 +470,6 @@ def run_b200(args) -> None:
     if dist is not None and not args.no_gather:
         # three output buffers: the persistent kernel holds every SM for the whole step, so the gather of step i only gets
         # SMs when step i+1's kernel drains; with two buffers step i+2 would then wait for that gather behind an idle GPU
-        # (measured at N = 2: 11.01 ms per step against 10.39 + 0.19 for kernel + collective)
         NB = 3
         y2 = [y_dev] + [torch.empty_like(y_dev) for _ in range(NB - 1)]
         gathered = [torch.empty((world,) + tuple(y_dev.shape), dtype=y_dev.dtype, device="cuda") for _ in range(NB)]
@@ -459,9 +487,8 @@ def run_b200(args) -> None:
                 dist.all_gather_into_tensor(gathered[b].view(-1), y2[b].view(-1))
                 done[b].record(side)
 
-        # The collective finds its SMs in the last, partly filled round of the persistent kernel (4096 streams over 296 CTAs =
-        # 13.8 rounds: 24 SMs idle for the last ~0.7 ms of a step).  Reserving SMs for it outright (nam_b200_set_reserved_sms)
-        # was measured and costs a whole extra round (4 SMs: 288 CTAs -> 15 rounds, +8 %), so none are reserved here.
+        # The collective finds its SMs in the last, partly filled round of the persistent kernel.  Reserving SMs for it
+        # outright (nam_b200_set_reserved_sms) can cost the kernel a whole extra round, so none are reserved here.
         for i in range(max(args.warmup, NB)):
             step_with_gather(i)
         barrier()
@@ -504,9 +531,7 @@ def run_b200(args) -> None:
         return
 
     # ---- the other configurations BASELINE.json names, device-resident, a few steps each (N = 1 only) ----
-    fp32_packed = nb.measure_fp32_tflops(local_rank, packed=True)
-    fp32_scalar = nb.measure_fp32_tflops(local_rank, packed=False)
-    fp32_peak = max(fp32_packed, fp32_scalar)  # the roof is the best FP32 FMA rate the SMs can be measured to issue
+    fp32_peak = nb.measure_fp32_tflops(local_rank, packed=False)  # the best FP32 FMA rate the SMs can be measured to issue
     secondary = None
     if world == 1 and not args.no_secondary and args.model == MODEL:
         secondary = {}
@@ -547,8 +572,8 @@ def run_b200(args) -> None:
         quick("wavenet_a1_standard_batch4096_128frame_calls", MODEL, 4096, 128, steps=32)
         quick("a2_full_batch4096", "a2_full", 4096, 4096, steps=4)
         quick("lstm_batch4096", "lstm", 4096, 4096, steps=4)
-        # latency roofline of the recurrence (SURVEY.md 8d: streams / step latency).  4096 streams are 512 warps on 592
-        # schedulers: every warp issues alone, so the step is bound by its dependent chain.  Chain of the gate-split
+        # latency roofline of the recurrence (SURVEY.md 8d: streams / step latency).  4096 streams are 512 warps on 528
+        # schedulers (132 SMs x 4): every warp issues alone, so the step is bound by its dependent chain.  Chain of the gate-split
         # kernel for a 1-layer cell (instruction latencies of the microarchitecture guide: FFMA / FMUL 4, SHFL ~25, MUFU.RCP
         # ~20): gate FMAs (1 + H + bias) x 4  ->  fast_tanh 45  ->  shuffle 25  ->  cell update 8  ->  fast_tanh 45  ->  h 4.
         if "error" not in secondary["lstm_batch4096"]:
@@ -556,12 +581,12 @@ def run_b200(args) -> None:
             H = 3
             chain_cycles = (1 + H + 1) * 4 + 45 + 25 + 8 + 45 + 4
             ns_big = big["ms_per_step"] * 1e6 / big["frames_per_step"]
-            ns_chain = chain_cycles / 1.965
+            ns_chain = chain_cycles / 1.98
             big["roofline"] = {"bound": "latency of one recurrence step", "ns_per_step": ns_big,
-                               "critical_path_cycles_estimate": chain_cycles, "critical_path_ns_at_1965MHz": ns_chain,
+                               "critical_path_cycles_estimate": chain_cycles, "critical_path_ns_at_1980MHz": ns_chain,
                                "frac": ns_chain / ns_big, "steps_per_s_per_stream": 1e9 / ns_big,
-                               "note": "serial in time: throughput = streams in flight / step latency (26 Gsamples/s = 4096 "
-                                       "streams / 155 ns); the FLOP fraction is not the bound"}
+                               "note": "serial in time: throughput = streams in flight / step latency; the FLOP fraction "
+                                       "is not the bound"}
         quick("wavenet_a2_max_batch4096_general_kernel", "wavenet_a2_max", 4096, 1024, steps=2)
 
     # ---- roofline of the fused kernel (one launch per step) ----
@@ -576,30 +601,19 @@ def run_b200(args) -> None:
         "peak": fp32_peak,
         "unit": "TFLOP/s",
         "frac": achieved_tf / fp32_peak if fp32_peak > 0 else None,
-        "peak_source": "max of the self-measured FP32 FMA issue rates on this GPU (nam_b200_measure_fp32_tflops): "
-                       f"scalar FFMA {fp32_scalar:.1f}, packed FFMA2 {fp32_packed:.1f} TFLOP/s; MEASURED_PEAKS.json "
-                       "carries no FP32 figure (nominal: 148 SMs x 128 FMA/clk x 1.965 GHz = 74.5)",
+        "peak_source": "self-measured FP32 FFMA issue rate on this GPU (nam_b200_measure_fp32_tflops); H100 SXM "
+                       "nominal: 132 SMs x 128 FMA/clk x 2 FLOP x 1.98 GHz = 66.9 TFLOP/s",
         "kernel": ("wavenet_spec_kernel (the model compiled by NVRTC at load: weights as FFMA immediates, history staged by "
                    "cp.async.bulk)" if jit_state == 1 else "wavenet_fused_kernel (precompiled, weights in shared memory)"),
         "jit": {"state": jit_state, "note": jit_note},
         "flops_per_launch": flops_per_launch,
         "kernel_ms": kernel_ms,
-        "traffic": None,
         "hbm": {"algorithmic_bytes_per_launch": alg_bytes, "achieved_GBs": alg_bytes / (kernel_ms * 1e-3) / 1e9,
                 "peak_GBs": peaks["hbm_gbs"], "frac": alg_bytes / (kernel_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
                 "of": peaks["_source"]},
         "tensor": {"frac_of_bf16_peak": achieved_tf / peaks["bf16_tflops"], "of": peaks["_source"],
                    "note": "kernel uses the FP32 FMA pipe, not tensor cores (1e-5 parity forbids TF32/BF16 operands)"},
     }
-    # DRAM bytes of one launch from the committed ncu --set full capture of this command's default shape
-    prof = ROOT / "profiles" / ("r02_traffic.json" if jit_state == 1 else "r01_traffic.json")
-    if prof.exists() and args.model == MODEL and (B, n) == (4096, 4096) and args.geometry == 0 and fast:
-        try:
-            t = json.loads(prof.read_text())
-            roofline["traffic"] = t.get("dram_bytes_per_launch_at_bench_shape")
-            roofline["traffic_source"] = t.get("source")
-        except Exception:
-            pass
 
     cpu = None
     if not args.no_cpu_baseline and world == 1 and rank == 0:  # reported at N = 1 only

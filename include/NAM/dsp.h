@@ -1,6 +1,6 @@
 // NAM/dsp.h -- drop-in replacement for the reference header of the same path, for the inference hot
 // path only: the nam::DSP interface (reference NAM/dsp.h:70-231) with the same public names, argument
-// meaning and error behaviour, backed by libnam_b200.so (hand-written sm_100a kernels behind the C ABI
+// meaning and error behaviour, backed by libnam_b200.so (hand-written sm_90a kernels behind the C ABI
 // of include/nam_b200.h) instead of Eigen.  No Eigen and no nlohmann types appear here, so a host that
 // only uses the public DSP surface (the reference's tools/benchmodel.cpp, tools/render.cpp,
 // tools/loadmodel.cpp, or the NeuralAmpModelerPlugin) compiles against it unchanged.
@@ -47,7 +47,7 @@ private:
 };
 
 /// Base class of all models.  The default process() copies input to output, exactly like the
-/// reference's (NAM/dsp.cpp:103-119); models loaded by get_dsp() are B200 subclasses.
+/// reference's (NAM/dsp.cpp:103-119); models loaded by get_dsp() are subclasses backed by libnam_b200.so.
 class DSP
 {
 public:
@@ -100,7 +100,7 @@ private:
   Level mOutputLevel;
 };
 
-/// A model whose process() runs on a B200 through libnam_b200.so.  One object == one stream of the
+/// A model whose process() runs on the GPU (H100, sm_90a) through libnam_b200.so.  One object == one stream of the
 /// handle (stream 0), so the reference's calling sequence get_dsp -> Reset -> process... works as is.
 class B200DSP : public DSP
 {

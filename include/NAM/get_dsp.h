@@ -1,4 +1,4 @@
-// NAM/get_dsp.h -- nam::get_dsp for the B200 library (reference NAM/get_dsp.h:66-122).
+// NAM/get_dsp.h -- nam::get_dsp for the libnam_b200.so library (reference NAM/get_dsp.h:66-122).
 #pragma once
 
 #include <filesystem>
@@ -41,7 +41,7 @@ std::unique_ptr<DSP> get_dsp(const std::filesystem::path config_filename, dspDat
 /// From the JSON text of a .nam document (the reference's nlohmann::json overload, without the dependency).
 std::unique_ptr<DSP> get_dsp_from_json_text(const std::string& nam_json_text, DspLoadOptions options = DspLoadOptions());
 
-/// B200 extension: a model carrying `batch` independent streams; use B200DSP::Handle() with
+/// Library extension: a model carrying `batch` independent streams; use B200DSP::Handle() with
 /// nam_b200_process_f32 for the batched entry point.
 std::unique_ptr<DSP> get_dsp_batched(const std::filesystem::path config_filename, int batch,
                                      DspLoadOptions options = DspLoadOptions());

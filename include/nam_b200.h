@@ -1,5 +1,5 @@
 /*
- * nam_b200.h -- C ABI of libnam_b200.so: NeuralAmpModelerCore's inference hot path on B200.
+ * nam_b200.h -- C ABI of libnam_b200.so: NeuralAmpModelerCore's inference hot path on H100 (sm_90a).
  *
  * The reference has no FFI of its own (it is a C++ static library); these entry points are what
  * a binding of its public surface for this path needs, one for one:
@@ -57,9 +57,9 @@ typedef struct nam_b200_options
   int32_t fast_tanh; /* 1 = Activation::enable_fast_tanh() was called before loading (benchmodel default) */
   int32_t prewarm_on_reset; /* 1 (reference default) = reset() prewarms; 0 = SetPrewarmOnReset(false) */
   int32_t ctas_per_sm; /* 0 = library default; tuning knob for the persistent WaveNet kernel */
-  int32_t kernel_geometry; /* WaveNet kernel: 0 = library default; 1 = FP32 FFMA2 kernel, 128-thread CTAs (tile 256);
-                              2 = FP32 FFMA2 kernel, 256-thread CTAs (tile 512); 3 = tensor-core kernel (tcgen05,
-                              3xTF32 split, tile 128); 4 = the general kernel (all WaveNet options, one CTA per stream,
+  int32_t kernel_geometry; /* WaveNet kernel: 0 = library default; 1 = FP32 FFMA kernel, 128-thread CTAs (tile 256);
+                              2 = FP32 FFMA kernel, 256-thread CTAs (tile 512); 3 = tensor-core kernel (none in
+                              this library: refused); 4 = the general kernel (all WaveNet options, one CTA per stream,
                               thread per frame) that otherwise serves only models outside the fused families */
   int32_t tile_mode; /* few streams x long calls (batch x tiles <= resident CTAs): 0 = library default: lock-step
                         tile-parallel mode (every (stream, tile) its own CTA, all tiles advancing layer by layer; a
@@ -161,16 +161,15 @@ int nam_b200_multi_process_f32(nam_b200_multi* mm, const float* in, float* out, 
 int nam_b200_process_f64_planar(nam_b200_model* m, const double* const* input, double* const* output, int n_frames);
 int nam_b200_process_f32_planar(nam_b200_model* m, const float* const* input, float* const* output, int n_frames);
 
-/* 1 when the library was built with the tcgen05 / TMEM WaveNet kernel (options.kernel_geometry = 3; a build option,
- * NAM_B200_BUILD_TC=1: validated to the same 1e-5 but slower than the FP32 kernels on the reference's model families), else 0:
- * creating a handle with kernel_geometry = 3 then fails with NAM_B200_ERR_UNSUPPORTED. */
+/* 1 when the library has a tensor-core WaveNet kernel (options.kernel_geometry = 3), else 0: creating a handle with
+ * kernel_geometry = 3 then fails with NAM_B200_ERR_UNSUPPORTED.  The sm_90a library has none (0). */
 int nam_b200_has_tensor_core_kernel(void);
 
 /* The persistent WaveNet throughput kernels occupy every SM for a whole call, so a concurrent kernel on another stream (an NCCL
  * collective gathering the previous call's outputs, say) only starts when they drain.  Leaving `n_sms` SMs free (0 = none,
  * the default) lets such work overlap the call.  The price is
  * quantised: the streams are walked in rounds of (CTAs per SM) x (SMs left), so check that the batch does not need one more
- * round (4096 streams, 2 CTAs per SM: 14 rounds on 147 or 148 SMs, 15 on 146 or fewer). */
+ * round (4096 streams, 2 CTAs per SM: 16 rounds on 128 to 132 SMs, 17 on 127 or fewer). */
 int nam_b200_set_reserved_sms(nam_b200_model* m, int n_sms);
 
 /* LSTM reads the fast-tanh switch at run time (NAM/lstm.cpp:48); WaveNet captured it at load. */
@@ -207,7 +206,7 @@ int nam_b200_inspect_file(const char* nam_path, int fast_tanh, char* out, int64_
  * GPU -- NVRTC cross-compiles -- and describe the outcome as a small JSON object: ok, from_cache, compile_seconds,
  * cubin_bytes, threads, frames_per_thread, smem_bytes, why_not.  Used to pre-populate the cache at install time. */
 int nam_b200_jit_prepare_json(const char* nam_json_text, int fast_tanh, char* out, int64_t capacity);
-/* The same for the kernel geometry a handle of `max_batch` streams on a 148-SM device would get (the short-call entry point
+/* The same for the kernel geometry a handle of `max_batch` streams on a 132-SM device (H100 SXM) would get (the short-call entry point
  * packs 6, 7 or 8 streams per CTA, whichever fills whole waves best at max_batch). */
 int nam_b200_jit_prepare_json_for_batch(const char* nam_json_text, int fast_tanh, int max_batch, char* out, int64_t capacity);
 /* Diagnostic: how this handle's specialised kernel was obtained, or why it has none.  Returns the text's length. */
@@ -224,8 +223,8 @@ int64_t nam_b200_submodel_json(const char* nam_json_text, int index, double* max
 /* Thread-local message of the last failing call on this thread. */
 const char* nam_b200_last_error(void);
 
-/* Measured FP32 FMA issue rate of the device (packed FFMA2 micro-benchmark), in TFLOP/s.  Used by
- * bench.py as the compute roofline for the fused kernel. Returns < 0 on error. */
+/* Measured FP32 FMA issue rate of the device (FFMA micro-benchmark), in TFLOP/s.  Used by bench.py as the compute
+ * roofline for the fused kernel.  `use_ffma2` is ignored: sm_90 has no packed FP32 FMA.  Returns < 0 on error. */
 double nam_b200_measure_fp32_tflops(int device, int use_ffma2);
 
 #ifdef __cplusplus

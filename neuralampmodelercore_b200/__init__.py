@@ -1,6 +1,6 @@
-"""neuralampmodelercore_b200 -- NeuralAmpModelerCore's per-sample inference hot path, B200-native.
+"""neuralampmodelercore_b200 -- NeuralAmpModelerCore's per-sample inference hot path, H100-native (sm_90a).
 
-The package holds only what the path needs: csrc/ (hand-written sm_100a kernels + the C ABI of
+The package holds only what the path needs: csrc/ (hand-written sm_90a kernels + the C ABI of
 include/nam_b200.h, built in-tree into lib/libnam_b200.so) and a thin Python mirror of the reference's
 nam::DSP / nam::get_dsp interface (dsp.py) used by tests and bench.py.
 """

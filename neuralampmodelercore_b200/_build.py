@@ -1,4 +1,4 @@
-"""In-tree build of libnam_b200.so with nvcc for sm_100a (no JIT cache, no torch extension machinery).
+"""In-tree build of libnam_b200.so with nvcc for sm_90a (H100) (no JIT cache, no torch extension machinery).
 
 The shared library is written to neuralampmodelercore_b200/lib/ so it travels with the repo snapshot
 to the GPU box; it is git-ignored (*.so) so history stays source-only.
@@ -17,22 +17,17 @@ LIB_PATH = LIB_DIR / "libnam_b200.so"
 INCLUDE = PKG.parent / "include"
 
 SOURCES = ["nam_b200.cu", "nam_model_spec.cpp", "json_lite.cpp", "wavenet_pack.cpp", "generic_pack.cpp", "nam_dsp_shim.cpp",
-           "jit_spec.cpp", "wavenet_tc_launch.cu"]
-
-
-def with_tc() -> bool:
-    """Build option: NAM_B200_BUILD_TC=1 compiles the tensor-core WaveNet kernel (wavenet_tc.cuh) into the library; the default
-    build carries stubs (DESIGN.md section 2.2: validated, slower than the FP32 kernels on the reference's model families)."""
-    return os.environ.get("NAM_B200_BUILD_TC", "0").strip().lower() in ("1", "true", "yes", "on")
+           "jit_spec.cpp"]
 
 
 def _obj_name(src: Path) -> str:
-    # the option is part of the object's name, so switching it recompiles / relinks the right one
-    return src.name + (".tc1.o" if src.name == "wavenet_tc_launch.cu" and with_tc() else ".o")
+    return src.name + ".o"
+
+GENCODE = "arch=compute_90a,code=sm_90a"
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    GENCODE,
     "-O3",
     "-lineinfo",
     "-std=c++17",
@@ -53,15 +48,8 @@ def sources() -> list[Path]:
     return [CSRC / s for s in SOURCES if (CSRC / s).exists()]
 
 
-def _options_stamp() -> str:
-    return f"tc={int(with_tc())}\n"
-
-
 def _stale() -> bool:
     if not LIB_PATH.exists():
-        return True
-    stamp = LIB_DIR / "build_options.txt"
-    if not stamp.exists() or stamp.read_text() != _options_stamp():
         return True
     t = LIB_PATH.stat().st_mtime
     deps = list(CSRC.glob("*")) + list(INCLUDE.rglob("*.h"))
@@ -93,8 +81,6 @@ def _embed(stem: str, ext: str = ".cuh") -> Path:
 
 def _compile_object(src: Path, obj: Path, verbose: bool) -> str:
     cmd = [_nvcc(), *[f for f in NVCC_FLAGS if f != "-shared"], f"-I{INCLUDE}", "-c", "-o", str(obj), str(src)]
-    if src.name == "wavenet_tc_launch.cu" and with_tc():
-        cmd.insert(1, "-DNAM_B200_WITH_TC=1")
     if verbose:
         cmd[1:1] = ["-Xptxas", "-v"]
     proc = subprocess.run(cmd, capture_output=True, text=True)
@@ -137,13 +123,12 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         logs = list(ex.map(lambda j: _compile_object(j[0], j[1], verbose), jobs))
     tmp = LIB_DIR / "libnam_b200.so.tmp"
-    cmd = [_nvcc(), "-shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(tmp),
+    cmd = [_nvcc(), "-shared", "-Xcompiler", "-fPIC", "-gencode", GENCODE, "-o", str(tmp),
            *[str(obj_dir / _obj_name(s)) for s in sources()], "-ldl"]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if proc.returncode != 0:
         raise RuntimeError("link failed:\n" + " ".join(cmd) + "\n" + proc.stdout + proc.stderr)
     os.replace(tmp, LIB_PATH)
-    (LIB_DIR / "build_options.txt").write_text(_options_stamp())
     if verbose:
         print("\n".join(logs))
     return LIB_PATH

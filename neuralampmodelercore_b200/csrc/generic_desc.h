@@ -1,7 +1,7 @@
 // generic_desc.h -- plain-data description of a WaveNet with the reference's full option set, shared by
 // the host packer (generic_pack.cpp) and the general kernel (wavenet_generic.cuh).
 //
-// The fused kernels (wavenet_fused.cuh, wavenet_tc.cuh) cover the model families that matter for throughput
+// The fused kernels (wavenet_fused.cuh, wavenet_spec.cuh) cover the model families that matter for throughput
 // (SURVEY.md 8a, 8f-1).  Everything else the reference's WaveNet can express -- gated / blended activations,
 // bottleneck != channels, grouped convolutions, head1x1, the eight FiLM sites, a condition_dsp sub-model, the
 // post-stack head (NAM/wavenet/model.cpp:19-103,183-393,777-910; NAM/film.h; NAM/gating_activations.h) -- runs

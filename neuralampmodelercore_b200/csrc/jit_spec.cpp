@@ -190,7 +190,7 @@ struct CompiledKernel
   double compile_seconds = 0.0;
 };
 
-// header + `#include "<kernel_file>"` -> sm_100a cubin, through the disk cache.  `env_override`: development aid, an
+// header + `#include "<kernel_file>"` -> sm_90a cubin, through the disk cache.  `env_override`: development aid, an
 // environment variable that names a file to use instead of the embedded kernel source.
 CompiledKernel compile_or_fetch(const std::string& tag, const std::string& header, const char* kernel_file,
                                 const char* embedded_source, const char* env_override, const std::vector<std::string>& defines,
@@ -204,7 +204,7 @@ CompiledKernel compile_or_fetch(const std::string& tag, const std::string& heade
     if (*e && read_file(e, txt))
       kernel_source.assign(txt.begin(), txt.end());
   }
-  std::string opts_text = "-arch=sm_100a -std=c++17 -default-device";
+  std::string opts_text = "-arch=sm_90a -std=c++17 -default-device";
   for (const std::string& d : defines)
     opts_text += " " + d;
   uint64_t h = 1469598103934665603ull;
@@ -244,7 +244,7 @@ CompiledKernel compile_or_fetch(const std::string& tag, const std::string& heade
     return r;
   }
   // -default-device: the layer loop is a generic lambda, which NVRTC would otherwise take for a host function
-  std::vector<const char*> copts = {"--gpu-architecture=sm_100a", "-std=c++17", "-lineinfo", "-default-device"};
+  std::vector<const char*> copts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device"};
   for (const std::string& d : defines)
     copts.push_back(d.c_str());
   rc = n.CompileProgram(prog, (int)copts.size(), copts.data());

@@ -2,7 +2,7 @@
 //
 // The reference builds a graph of Eigen objects per model at load time (NAM/wavenet/model.cpp:580-683); this library's
 // throughput path goes one step further and compiles the model: NVRTC turns wavenet_spec.cuh + a generated header
-// (layer table as constexpr data, weights as `__device__ const float[]`) into sm_100a SASS in which every weight is the
+// (layer table as constexpr data, weights as `__device__ const float[]`) into sm_90a SASS in which every weight is the
 // immediate operand of an FFMA.  The cubin is cached on disk, keyed by a hash of everything that went into it.
 // Host only; no CUDA runtime types in this header.
 #pragma once

@@ -2,7 +2,7 @@
 // (reference: NAM/lstm.cpp:31-68 LSTMCell::process_, :136-168 LSTM::_process_sample).
 //
 // The recurrence is serial in time, so throughput = streams in flight / latency of one step.  A thread per stream
-// (lstm_kernel in nam_b200.cu, kept as the fallback for hidden sizes above 64) leaves a B200 almost idle at 4096
+// (lstm_kernel in nam_b200.cu, kept as the fallback for hidden sizes above 64) leaves most of the GPU idle at 4096
 // streams and walks the whole 4H x (I+H) matvec plus 5H activations in one dependent chain.  Here a group of
 // G = 4 / 8 / 16 / 32 lanes (the next power of two >= H, at most 32) owns a stream: lane u computes the four gate
 // pre-activations of hidden unit u (and u + 32 when H > 32), reads the other units' h through warp shuffles and

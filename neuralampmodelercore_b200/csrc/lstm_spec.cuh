@@ -1,4 +1,4 @@
-// lstm_spec.cuh -- the MODEL-SPECIALISED LSTM kernel for sm_100a (small cells: sum over layers of 4H(I+H) <= ~300 FMAs).
+// lstm_spec.cuh -- the MODEL-SPECIALISED LSTM kernel for sm_90a (small cells: sum over layers of 4H(I+H) <= ~300 FMAs).
 //
 // Compiled per model by NVRTC (jit_spec.cpp) together with a generated header that defines namespace `spec`: H, L, I as
 // constexpr and the weights as bit patterns read through spec::w(i).  What it computes (reference, under NAM/):
@@ -153,8 +153,8 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
           }
         if constexpr (FAST)
         {
-          // scalar on purpose: packed f32x2 evaluation (two activations per instruction) measured SLOWER here (315 vs
-          // 276 ns per step): a lone warp per scheduler is bound by the dependent chain, and FFMA2 has the longer one
+          // scalar on purpose: a lone warp per scheduler is bound by the dependent chain, which pairing the activations
+          // does not shorten
 #pragma unroll
           for (int u = 0; u < H; u++)
           {
@@ -210,8 +210,8 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
 }
 
 // ---- gate-split variant: FOUR lanes per stream, lane q = gate q (i, f, g, o) ----------------------------------------------
-// One thread per stream issues ~290 instructions per step from a single warp per scheduler (542 cycles measured for
-// lstm.nam); the step's dependent chain is only ~150.  Here lane q of a group of four computes gate q's H
+// One thread per stream issues ~290 instructions per step from a single warp per scheduler; the step's dependent chain is
+// only ~150 cycles.  Here lane q of a group of four computes gate q's H
 // pre-activations (its rows of W in registers: the rows differ per lane, so they cannot be immediates) and their
 // activation; the 4H activated values are exchanged by shuffles and every lane updates (c, h) of all units redundantly,
 // so nothing has to be broadcast back: ~115 instructions per lane per step, 8 streams per warp.

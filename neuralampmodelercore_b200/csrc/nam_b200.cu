@@ -1,5 +1,5 @@
 // nam_b200.cu -- C ABI of libnam_b200.so (include/nam_b200.h): model handles, device state,
-// kernel launches.  Host code is C++; every hot-path operation is a hand-written sm_100a kernel
+// kernel launches.  Host code is C++; every hot-path operation is a hand-written sm_90a kernel
 // (wavenet_fused.cuh, and the LSTM / Linear kernels below).  There is deliberately no CPU
 // fallback anywhere in this file.
 #include "../../include/nam_b200.h"
@@ -21,7 +21,6 @@
 #include "wavenet_fused.cuh"
 #include "wavenet_lat2.cuh"
 #include "wavenet_pack.h"
-#include "wavenet_tc_launch.h"
 #include "generic_pack.h"
 #include "wavenet_generic.cuh"
 #include "jit_spec.h"
@@ -317,8 +316,8 @@ __global__ void broadcast_state_kernel(float* __restrict__ state, long stride_fl
   }
 }
 
-// FP32 FMA issue-rate micro-benchmark: 8 independent accumulator pairs per thread.
-template <bool PACKED>
+// FP32 FMA issue-rate micro-benchmark: 8 independent accumulator pairs per thread (sm_90 has no packed FP32 FMA, so
+// every pair is two scalar FFMAs).
 __global__ void __launch_bounds__(256) fma_peak_kernel(float* out, int iters, float seed)
 {
   float2 a[8];
@@ -332,13 +331,8 @@ __global__ void __launch_bounds__(256) fma_peak_kernel(float* out, int iters, fl
 #pragma unroll
     for (int i = 0; i < 8; i++)
     {
-      if (PACKED)
-        a[i] = __ffma2_rn(a[i], m, c);
-      else
-      {
-        a[i].x = fmaf(a[i].x, m.x, c.x);
-        a[i].y = fmaf(a[i].y, m.y, c.y);
-      }
+      a[i].x = fmaf(a[i].x, m.x, c.x);
+      a[i].y = fmaf(a[i].y, m.y, c.y);
     }
   }
   float s = 0.0f;
@@ -382,8 +376,7 @@ struct nam_b200_model
   size_t hist_floats = 0;
   int wn_ctas_ls[3] = {0, 0, 0}; // resident CTAs per SM of the lock-step kernels (kLsGeom)
   int wn_ctas_short[2] = {0, 0}; // same for the short-call (multi-stream tile) geometries 2 / 3
-  int wn_geometry = 1; // 0 / 1: index into kWnGeom (FFMA kernel); 2: tensor-core kernel (wavenet_tc.cuh)
-  float* d_tc_blob = nullptr; // per-layer B-operand images of the tensor-core kernel
+  int wn_geometry = 1; // 0 / 1: index into kWnGeom (FFMA kernel)
   // model-specialised kernel (wavenet_spec.cuh compiled for this model by NVRTC, jit_spec.cpp): the throughput path
   cudaLibrary_t spec_lib = nullptr;
   cudaLibrary_t spec_lib_extra = nullptr; // second program of the model: the 128- / 256-frame short-call entry points
@@ -450,8 +443,6 @@ struct nam_b200_model
     cudaSetDevice(device);
     if (d_weights)
       cudaFree(d_weights);
-    if (d_tc_blob)
-      cudaFree(d_tc_blob);
     if (d_glayers)
       cudaFree(d_glayers);
     if (spec_lib)
@@ -539,9 +530,8 @@ int occupancy_wavenet_variant(size_t smem)
 //   LS geometry 1: 256 threads x 2 frames, tile 512, >= 2 CTAs/SM  (kernel_geometry 2; also when tile 256 does not fit)
 //   LS geometry 2: 128 threads x 1 frame, tile 128: only while every CTA has an SM to itself (batch x tiles <= SMs:
 //                  one stream in 4096-frame calls), where a layer step is as long as one warp's instruction stream
-// (A 256 x 1 geometry -- half the instructions per thread and layer step, twice the warps per tile -- measured slower
-// on both shapes that matter: 37.2 vs 41.2 Msamples/s for one stream in 4096-frame calls, 437 vs 487 for one
-// 96,000-frame call: the weight loads per FFMA2 double.)
+// (A 256 x 1 geometry -- half the instructions per thread and layer step, twice the warps per tile -- doubles the weight
+// loads per FMA.)
 struct LsGeometry
 {
   int nt, s, min_ctas, lq;
@@ -770,7 +760,7 @@ bool wavenet_ls_candidate(const nam_b200_model* m, int g)
 // co-resident, -1 if none.
 int wavenet_ls_geometry(nam_b200_model* m, int batch, int n_frames, int* tiles_out)
 {
-  if (m->opts.tile_mode != 0 || m->wn_geometry > 1 || m->use_generic)
+  if (m->opts.tile_mode != 0 || m->use_generic)
     return -1;
   static const int order[kLsGeoms] = {2, 0, 1};
   for (int oi = 0; oi < kLsGeoms; oi++)
@@ -794,7 +784,7 @@ int wavenet_ls_geometry(nam_b200_model* m, int batch, int n_frames, int* tiles_o
 // lock-step mode can serve, so that process() never allocates
 void ensure_hist(nam_b200_model* m)
 {
-  if (m->spec.arch != Arch::WaveNet || m->use_generic || m->wn_geometry > 1 || m->opts.tile_mode != 0)
+  if (m->spec.arch != Arch::WaveNet || m->use_generic || m->opts.tile_mode != 0)
     return;
   const int planes = wavenet_hist_planes(m->plan);
   size_t need = 0, need_flags = 0;
@@ -871,8 +861,8 @@ struct GenSpecKernelParams // mirror of namb200_gspec::GParams
 
 
 // Geometry of the specialised kernel for a handle of `max_batch` streams.  Streams per CTA of the short-call entry point:
-// the count that fills whole waves of 2 CTAs per SM best (4096 streams: 8 per CTA = 512 CTAs = 1.73 waves, 7 per CTA = 586 =
-// 1.98 waves).
+// the count that fills whole waves of 2 CTAs per SM best (4096 streams on 132 SMs: 8 per CTA = 512 CTAs = 1.94 waves, 7 per
+// CTA = 586 = 2.22 waves).
 SpecGeometry spec_geometry_for(int max_batch, int sm_count)
 {
   SpecGeometry g;
@@ -1012,7 +1002,7 @@ struct LatKernelParams // mirror of namb200_lat::LatParams
 // 64 / 128 frames.  Wanted when jit is "required" or "preferred" (the C++ shim's default), never by the automatic policy.
 void setup_lat_kernel(nam_b200_model* m)
 {
-  if (m->spec.arch != Arch::WaveNet || m->use_generic || m->wn_geometry > 1 || m->opts.kernel_geometry != 0)
+  if (m->spec.arch != Arch::WaveNet || m->use_generic || m->opts.kernel_geometry != 0)
     return;
   const int mode = jit_mode(m);
   if (!(mode == 1 || mode == 3) || m->opts.max_batch > m->sm_count || m->max_frames > 128)
@@ -1151,32 +1141,13 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
     kp.layers[i] = plan.layers[i];
   const int geom = m->wn_geometry;
   const int c0 = plan.cp[0], c1 = plan.n_arrays > 1 ? plan.cp[1] : 0;
-  if (geom == 2)
-  {
-    // tensor-core variant (wavenet_tc.cuh)
-    kp.tc_blob = m->d_tc_blob;
-    for (size_t i = 0; i < plan.layers.size(); i++)
-    {
-      kp.tc_off[i] = plan.tc_off[i];
-      kp.tc_floats[i] = plan.tc_floats[i];
-    }
-    const size_t smem_tc = tc_smem_bytes(plan);
-    if (m->wn_ctas_per_sm <= 0)
-      m->wn_ctas_per_sm = m->opts.ctas_per_sm > 0 ? m->opts.ctas_per_sm : tc_occupancy(c0, c1, smem_tc);
-    int grid_tc = std::min(batch, m->wn_ctas_per_sm * m->sm_count);
-    if (grid_tc < 1)
-      grid_tc = 1;
-    tc_launch(c0, c1, kp, (int)((plan.tc_max_image_floats + 3) / 4), (int)plan.layers.size(), grid_tc, smem_tc, st);
-    m->launches++;
-    return;
-  }
   // few streams, short calls: the precompiled low-latency kernel (wavenet_lat2.cuh): one CTA per stream, the weight blob and
   // every history window of the call brought in by bulk copies at kernel start ($NAM_B200_LAT_KERNEL=jit: prefer the
   // model-specialised wavenet_lat.cuh where the handle has it, =off: neither)
   {
     const char* lat_env = std::getenv("NAM_B200_LAT_KERNEL"); // (read per call: tests switch it)
-    // 0: the model-specialised kernel where the handle has it (20.5 us per 64-frame call of a1_standard), else the
-    // precompiled one (29 us; the 128 x 1 geometry it replaces: 41.6); "precompiled" / "jit" / "off" pin the choice
+    // 0: the model-specialised kernel where the handle has it, else the precompiled one (both faster than the 128 x 1
+    // geometry they replace); "precompiled" / "jit" / "off" pin the choice
     const int lat_pref = !lat_env ? 0 : (std::strcmp(lat_env, "jit") == 0 ? 1 : (std::strcmp(lat_env, "off") == 0 ? 2 : (std::strcmp(lat_env, "precompiled") == 0 ? 3 : 0)));
     const int fw = n_frames <= 64 ? 2 : 4;
     const bool jit_lat_ok = lat_pref != 2 && lat_pref != 3 && m->lat_state == 1 && n_frames <= m->lat_frames && batch <= m->sm_count;
@@ -1408,9 +1379,9 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
     LstmSpecKernelParams sp{m->d_state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames};
     void* args[] = {&sp};
     // The step rate is bound by one warp's instruction stream as long as every warp has a scheduler to itself: four
-    // lanes per stream (gate-split, 8 streams per warp: 155 ns per step for lstm.nam) while every warp still gets a
-    // scheduler of its own (4 x SMs), else one thread per stream (32 per warp, 284 ns per step; measured at 16,384
-    // streams: 57.7 against 46.7 Gsamples/s).  kernel_geometry 1 / 2 pins one of them.
+    // lanes per stream (gate-split, 8 streams per warp: a shorter dependent chain per step) while every warp still gets a
+    // scheduler of its own (4 x SMs), else one thread per stream (32 per warp: more streams in flight).  kernel_geometry
+    // 1 / 2 pins one of them.
     const bool gates = m->spec.lstm.hidden >= 2
                        && (m->opts.kernel_geometry == 1 || (m->opts.kernel_geometry != 2 && (batch + 7) / 8 <= 4 * m->sm_count));
     if (gates)
@@ -1792,26 +1763,12 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
         m->state_stride = m->plan.state_floats;
         m->flops_per_frame = 2.0 * m->plan.macs_per_frame;
         m->variant = m->plan.cp[0] * 100 + (m->plan.n_arrays > 1 ? m->plan.cp[1] : 0);
-        // option: 0 default, 1 = FFMA 128-thread, 2 = FFMA 256-thread, 3 = tensor-core (tcgen05)
+        // option: 0 default, 1 = FFMA 128-thread, 2 = FFMA 256-thread, 3 = tensor-core (none on sm_90a)
         if (m->opts.kernel_geometry == 3)
-        {
-          if (!tc_built())
-            return fail(NAM_B200_ERR_UNSUPPORTED,
-                        "tensor-core kernel: this library was built without it (rebuild with NAM_B200_BUILD_TC=1; it is slower "
-                        "than the FP32 kernels on 8/16-channel models, DESIGN.md section 2.2)");
-          if (!m->plan.tc_eligible)
-            return fail(NAM_B200_ERR_UNSUPPORTED, "tensor-core kernel not available for this model: " + m->plan.tc_why_not);
-          m->wn_geometry = 2;
-          m->state_stride = 2 * m->plan.state_floats; // this kernel's rings hold hi and lo parts (wavenet_tc.cuh)
-          if (tc_smem_bytes(m->plan) > 227 * 1024)
-            return fail(NAM_B200_ERR_UNSUPPORTED, "tensor-core kernel: tiles do not fit in shared memory");
-          CUDA_CHECK(cudaMalloc(&m->d_tc_blob, m->plan.tc_blob.size() * sizeof(float)));
-          CUDA_CHECK(cudaMemcpy(m->d_tc_blob, m->plan.tc_blob.data(), m->plan.tc_blob.size() * sizeof(float),
-                                cudaMemcpyHostToDevice));
-        }
-        else
-          m->wn_geometry = (m->opts.kernel_geometry == 1) ? 0 : 1;
-        if (m->wn_geometry < 2 && wavenet_smem_bytes(m->plan, m->wn_geometry) > 227 * 1024)
+          return fail(NAM_B200_ERR_UNSUPPORTED, "tensor-core WaveNet kernel: this sm_90a library has none (use kernel_geometry "
+                                                "0, 1, 2 or 4)");
+        m->wn_geometry = (m->opts.kernel_geometry == 1) ? 0 : 1;
+        if (wavenet_smem_bytes(m->plan, m->wn_geometry) > 227 * 1024)
           return fail(NAM_B200_ERR_UNSUPPORTED, "WaveNet weights do not fit in shared memory");
         setup_spec_kernel(m.get());
         break;
@@ -2235,7 +2192,7 @@ int nam_b200_jit_prepare_json_for_batch(const char* nam_json_text, int fast_tanh
     {
       const WaveNetPlan wp = plan_wavenet(ms);
       fused_family = wp.eligible && ms.in_channels == 1 && ms.out_channels == 1;
-      b = fused_family ? build_spec_kernel(wp, spec_geometry_for(std::max(max_batch, 1), 148))
+      b = fused_family ? build_spec_kernel(wp, spec_geometry_for(std::max(max_batch, 1), 132))  // H100 SXM
                        : build_generic_spec_kernel(plan_generic(ms)); // every other WaveNet: the general kernel, compiled
     }
     // WaveNets: also the low-latency kernel for 64-frame calls (the plugin protocol), so that a first Reset finds it cached
@@ -2690,7 +2647,7 @@ int nam_b200_process_f64_planar(nam_b200_model* m, const double* const* input, d
 
 int nam_b200_has_tensor_core_kernel(void)
 {
-  return tc_built() ? 1 : 0;
+  return 0; // no tensor-core WaveNet kernel on sm_90a
 }
 
 int nam_b200_set_reserved_sms(nam_b200_model* m, int n_sms)
@@ -2786,7 +2743,7 @@ double nam_b200_last_kernel_ms(nam_b200_model* m)
   return (double)ms;
 }
 
-double nam_b200_measure_fp32_tflops(int device, int use_ffma2)
+double nam_b200_measure_fp32_tflops(int device, int /*use_ffma2: no packed FP32 FMA on sm_90*/)
 {
   try
   {
@@ -2806,10 +2763,7 @@ double nam_b200_measure_fp32_tflops(int device, int use_ffma2)
     for (int rep = 0; rep < 5; rep++)
     {
       CUDA_CHECK(cudaEventRecord(e0));
-      if (use_ffma2)
-        fma_peak_kernel<true><<<blocks, threads>>>(d, iters, 1.0f);
-      else
-        fma_peak_kernel<false><<<blocks, threads>>>(d, iters, 1.0f);
+      fma_peak_kernel<<<blocks, threads>>>(d, iters, 1.0f);
       CUDA_CHECK(cudaEventRecord(e1));
       CUDA_CHECK(cudaEventSynchronize(e1));
       float ms = 0.0f;

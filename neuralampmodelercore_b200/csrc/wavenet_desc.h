@@ -81,28 +81,10 @@ struct WaveNetKernelParams
   long hist_stride; // floats per stream = total planes * hist_cols * 4
   int hist_cols; // tiles_per_stream * frames per tile
   int hist_plane0[kMaxArrays]; // first plane of array a: its layers' inputs, P planes each, then its head-conv input
-  // tensor-core variant (wavenet_tc.cuh): per-layer shared-memory images of the B operands
-  const float* tc_blob;
-  int tc_off[kMaxLayers]; // float offset of layer i's image in tc_blob
-  int tc_floats[kMaxLayers]; // its size (multiple of 4)
   // low-latency kernel (wavenet_lat2.cuh): completion doorbell, a word of mapped host memory that receives done_seq once the
   // call's outputs are visible to the host (nullptr: none)
   unsigned* done_flag;
   unsigned done_seq;
 };
-
-// Layout of one layer's tensor-core image (floats), CP = padded channels (8 or 16), KS = CP/8 K-steps:
-//   conv_hi [K][KS][2 chunks][16 n][4]   TF32-rounded weights, K-major "no swizzle" UMMA layout
-//   conv_lo [K][KS][2][16][4]            residuals w - hi
-//   p_hi    [KS][2][16][4]               layer1x1
-//   p_lo    [KS][2][16][4]
-//   vec     b[16] | M[16] | p[16] | slopes[16]
-constexpr int kTcTile = 128; // floats of one (tap, K-step) B tile: 2 chunks x 16 n x 4
-constexpr int kTcVec = 64;
-inline int tc_image_floats(int kernel, int cp)
-{
-  const int ks = cp / 8;
-  return (2 * kernel * ks + 2 * ks) * kTcTile + kTcVec;
-}
 
 } // namespace namb200

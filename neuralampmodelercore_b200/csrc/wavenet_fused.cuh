@@ -1,4 +1,4 @@
-// wavenet_fused.cuh -- the fused WaveNet layer-array kernel for sm_100a.
+// wavenet_fused.cuh -- the fused WaveNet layer-array kernel for sm_90a.
 //
 // What it replaces (reference file:line, all under NAM/):
 //   wavenet/model.cpp:822-910   WaveNet::process            (whole kernel)
@@ -24,8 +24,8 @@
 // thread's 16-byte vector load of (time, 4 channels) is contiguous across the warp's 32
 // consecutive time steps (conflict-free LDS.128 / fully coalesced LDG.128), at ANY tap
 // offset.  Weights live in shared memory as [in][out] rows so one warp-uniform LDS.128 yields 4
-// output-channel weights, consumed by packed FFMA2 (fma.rn.f32x2: two output channels per
-// instruction, input sample broadcast).
+// output-channel weights, consumed two output channels at a time (a register pair, input sample
+// broadcast; two scalar FFMAs on sm_90).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -191,8 +191,7 @@ __device__ __forceinline__ void tile_publish(const TileSync& ts, int step)
 // that follow; lanes 0..m-1 poll one predecessor each.
 constexpr int kLsFinalStep = 1 << 20;
 // Spin on a flag with acquire loads.  (Relaxed loads in the loop plus one fence.acq_rel.gpu at the end -- to avoid the
-// L1 invalidation each ld.acquire costs, profiles/r01h_lockstep_* -- measured SLOWER: 407 vs 487 Msamples/s for one
-// 96,000-frame stream; the fence waits for far more than the flag.)
+// L1 invalidation each ld.acquire costs -- was slower: the fence waits for far more than the flag.)
 __device__ __forceinline__ void ls_spin_until_above(const int* flag, const int step)
 {
   int v;
@@ -205,8 +204,7 @@ __device__ __forceinline__ void ls_publish_wait(const TileSync& ts, const int st
 {
   // The CTA's hist stores are ordered before the barrier, the barrier before thread 0's release: the release is
   // cumulative over everything that happens-before it, so one fence (inside st.release.gpu) covers the whole CTA's
-  // stores -- the pattern of a cooperative-groups grid barrier.  (A __threadfence() per thread here cost 10 % of the
-  // issue-stall cycles, profiles/r01h_lockstep_*: membar.)
+  // stores -- the pattern of a cooperative-groups grid barrier, cheaper than a __threadfence() per thread.
   __syncthreads();
   if (threadIdx.x == 0)
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(ts.mine), "r"(step + 1) : "memory");
@@ -215,11 +213,11 @@ __device__ __forceinline__ void ls_publish_wait(const TileSync& ts, const int st
   __syncthreads();
 }
 
-// ---- packed fp32 pairs ------------------------------------------------------------------------
-// Accumulators are kept as 64-bit register pairs and updated IN PLACE with fma.rn.f32x2 (SASS
-// FFMA2) through inline PTX: the "+l" constraint pins destination == addend, which stops ptxas
-// from rotating the accumulators through fresh registers (and paying one MOV per accumulator per
-// loop trip, 15% of all issued instructions in the first version of this kernel; profiles/).
+// ---- fp32 pairs ---------------------------------------------------------------------------------
+// Accumulators and epilogue values are kept as 64-bit register pairs (two output channels, or two
+// values of the element-wise math).  sm_90 has no packed FP32 arithmetic, so every pair operation is
+// two scalar round-to-nearest instructions on the halves: the same numbers fma.rn.f32x2 /
+// mul.rn.f32x2 / add.rn.f32x2 give, and ptxas keeps the halves in the register pair (no MOVs).
 typedef unsigned long long u64;
 
 __device__ __forceinline__ u64 pack2(const float lo, const float hi)
@@ -232,49 +230,41 @@ __device__ __forceinline__ void unpack2(const u64 v, float& lo, float& hi)
 {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
-__device__ __forceinline__ void fma2_acc(u64& acc, const u64 w, const u64 xx)
-{
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(w), "l"(xx));
-}
-__device__ __forceinline__ void add2_acc(u64& acc, const u64 v)
-{
-  asm("add.rn.f32x2 %0, %0, %1;" : "+l"(acc) : "l"(v));
-}
-
-// ---- packed fp32 pair arithmetic for the element-wise epilogue math (halves its issue slots) ----
 __device__ __forceinline__ u64 tc_fma2(u64 a, u64 b, u64 c)
 {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float al, ah, bl, bh, cl, ch;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  unpack2(c, cl, ch);
+  return pack2(__fmaf_rn(al, bl, cl), __fmaf_rn(ah, bh, ch));
 }
 __device__ __forceinline__ u64 tc_mul2(u64 a, u64 b)
 {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float al, ah, bl, bh;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  return pack2(__fmul_rn(al, bl), __fmul_rn(ah, bh));
 }
 __device__ __forceinline__ u64 tc_add2(u64 a, u64 b)
 {
-  u64 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float al, ah, bl, bh;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  return pack2(__fadd_rn(al, bl), __fadd_rn(ah, bh));
+}
+__device__ __forceinline__ void fma2_acc(u64& acc, const u64 w, const u64 xx)
+{
+  acc = tc_fma2(w, xx, acc);
+}
+__device__ __forceinline__ void add2_acc(u64& acc, const u64 v)
+{
+  acc = tc_add2(acc, v);
 }
 __device__ __forceinline__ u64 tc_dup(float v)
 {
   return pack2(v, v);
 }
 constexpr u64 kTcAbsMask = 0x7FFFFFFF7FFFFFFFull;
-// x = hi + lo with hi on 11 significant bits (exactly a TF32 number), Veltkamp's splitting: 4 packed instructions
-// per pair instead of 6 integer / float ones
-__device__ __forceinline__ void tc_split2(u64 x, u64& hi, u64& lo)
-{
-  const u64 m1 = tc_dup(-1.0f);
-  const u64 t = tc_mul2(x, tc_dup(8193.0f)); // 2^13 + 1
-  const u64 d = tc_fma2(m1, x, t); // t - x
-  hi = tc_fma2(m1, d, t); // t - (t - x)
-  lo = tc_fma2(m1, hi, x); // x - hi, exact
-}
 // the reference's rational fast_tanh (activations.h:91-98) on a pair
 __device__ __forceinline__ u64 tc_fast_tanh2(u64 x)
 {
@@ -292,7 +282,7 @@ __device__ __forceinline__ u64 tc_fast_tanh2(u64 x)
   return tc_mul2(num, pack2(rcp_approx(dl), rcp_approx(dh)));
 }
 
-// acc[o] += w_row[o] * x for C outputs, two per FFMA2 (x broadcast to both halves).
+// acc[o] += w_row[o] * x for C outputs, two per register pair (x broadcast to both halves).
 template <int C>
 __device__ __forceinline__ void axpy_row(u64 (&acc)[C / 2], const float* __restrict__ w_row, const float x)
 {

@@ -87,10 +87,9 @@ __device__ __forceinline__ void g_act_vec(const GenThread& c, const GAct& A, con
 // chains of a group are independent, one weight load feeds four of them); the bias, when given, is added once the sum
 // is complete -- the reference's order (conv1d.cpp:769, dsp.cpp:832-834).  The models that reach this kernel are narrow
 // (wavenet_a2_max.nam: 3..8 wide), so the input loop is kept rolled: an unrolled-by-8 loop with its remainder
-// handling cost more instructions than the arithmetic (profiles/r01h_general_kernel_*: FFMA 14 % of the issue slots).
-// (Taking this and the other helpers out of line shrinks the kernel from 22,000 to 3,700 instructions -- the profile
-// shows instruction-fetch stalls, profiles/r01i_general_kernel_* -- but measured slower, 768 vs 819 Msamples/s on
-// wavenet_a2_max.nam: the calls and the generic-address loads of the local vectors cost more than the fetches.)
+// handling cost more instructions than the arithmetic.
+// (Taking this and the other helpers out of line shrinks the kernel several times over, but was slower: the calls and
+// the generic-address loads of the local vectors cost more than the instruction fetches they save.)
 __device__ __forceinline__ void g_accumulate(const float* __restrict__ wt, const int in, const int op, const float* x,
                                              float* y, const bool from_zero, const float* __restrict__ bias)
 {

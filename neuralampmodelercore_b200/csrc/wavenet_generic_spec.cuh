@@ -1,8 +1,8 @@
 // wavenet_generic_spec.cuh -- the general WaveNet kernel (wavenet_generic.cuh), compiled PER MODEL by NVRTC.
 //
 // wavenet_generic.cuh interprets descriptors at run time: loop bounds come from memory, every per-frame vector is a local
-// array indexed by loop variables (local memory), weights are fetched from shared memory -- FFMA 13 % of the issue slots,
-// 0.82 Gsamples/s on wavenet_a2_max.nam (profiles/r01i_general_kernel_*).  Here the SAME algorithm, the same summation
+// array indexed by loop variables (local memory), weights are fetched from shared memory: bookkeeping, not arithmetic,
+// fills the issue slots.  Here the SAME algorithm, the same summation
 // order and the same ring layout are compiled together with a generated header (jit_spec.cpp) that holds the model as
 // constant data: `gspec::net`, `gspec::cond`, `gspec::layers[]` (the descriptors of generic_desc.h) and the weights as bit
 // patterns.  Every function below is force-inlined and every loop has, after inlining, a constant trip count, so the

@@ -1,9 +1,9 @@
-// wavenet_lat.cuh -- the MODEL-SPECIALISED LOW-LATENCY WaveNet kernel for sm_100a: few streams, short calls.
+// wavenet_lat.cuh -- the MODEL-SPECIALISED LOW-LATENCY WaveNet kernel for sm_90a: few streams, short calls.
 //
 // The reference's hosts call DSP::process() with ONE stream and 64-frame blocks (tools/benchmodel.cpp:116-133,
 // NeuralAmpModelerPlugin): such a call is pure latency.  The precompiled kernel walks it with one frame per thread of a
 // 128-thread CTA (half of them idle at 64 frames), ~22 layer steps each as long as one warp's whole instruction stream
-// for a layer: 41.6 us of kernel time per 64-frame call of wavenet_a1_standard.nam (profiles/r02c_latency_probe_before.log).
+// for a layer.
 //
 // This kernel is compiled per model by NVRTC like wavenet_spec.cuh (same generated header: namespace `spec`, weights as
 // FFMA immediates) and cuts the step three ways:
@@ -37,8 +37,8 @@ using namespace namb200_spec;
 #define NAMB200_LAT_GROUPS 4
 #endif
 // Channel groups.  Each group is its own instruction stream, and streaming straight-line code from L2 is what bounds this
-// kernel: one SM fetches ~10.6 B / cycle for 4 distinct streams but ~17.5 B / cycle for 8 (tools/ifetch_probe,
-// profiles/r02x_ifetch_probe.jsonl), so 8 groups of half-size streams finish sooner than 4.
+// kernel: an SM fetches more bytes per cycle from more distinct code streams, so 8 groups of half-size streams finish
+// sooner than 4.
 constexpr int kGroups = NAMB200_LAT_GROUPS;
 static_assert(kGroups == 4 || kGroups == 8, "4 or 8 channel groups");
 
@@ -205,7 +205,7 @@ __device__ __forceinline__ void ring_store_slice(const Ctx& c, const int g, cons
 
 // Every history window of the call, requested at kernel start.  Warp w takes the layers w, w + NW, ..: a bulk copy is issued
 // through uniform registers, one at a time per warp (~40 cycles each), and a1_standard has 160 of them -- spread over the
-// CTA's warps they cost 0.4 us instead of 3.
+// CTA's warps they cost a fraction of what one warp issuing them all would.
 template <int F, int NWARPS>
 __device__ __forceinline__ void request_all_history(const Ctx& c, const int warp, const int lane)
 {
@@ -417,7 +417,7 @@ __device__ __forceinline__ void wavenet_lat_body(const LatParams& p)
   {
     // barrier, then ONE system-scope fence by the signalling thread (fences are cumulative: it orders every output store the
     // barrier made it observe before the doorbell -- the grid-sync idiom); a fence by every thread before the barrier as well
-    // only put a second ~2.5 us system fence on the critical path (profiles/r02ze_*: `membar` 1.8 cycles per instruction)
+    // only puts a second system-scope fence on the critical path
     __syncthreads();
     if (tid == 0 && blockIdx.x == 0)
     {

@@ -3,12 +3,12 @@
 // Reference path: the same as wavenet_fused.cuh (NAM/wavenet/model.cpp:822-910, :463-549, :183-393; conv1d.cpp:666-683;
 // ring_buffer.cpp:7-109; dsp.cpp:436-836; activations.h:59-133).
 //
-// What the profiles of its two predecessors say about ONE stream x 64 frames of wavenet_a1_standard.nam:
-//   * the 128 x 1 geometry of wavenet_fused.cuh: 41.6 us of kernel time -- ~22 layer steps, each one warp's whole
+// What limits its two predecessors on ONE stream x 64 frames of wavenet_a1_standard.nam:
+//   * the 128 x 1 geometry of wavenet_fused.cuh: ~22 layer steps, each one warp's whole
 //     instruction stream for a layer, half the CTA idle at 64 frames, the L2 round trip of the ring columns paid per layer;
 //   * the model-specialised wavenet_lat.cuh (weights as FFMA immediates, output channels split over four warp groups, all
-//     history requested at kernel start): 20.5 us, and ncu names the bound: `no_instruction`, 12 cycles per issued
-//     instruction -- 313 KB of straight-line code executed exactly once per call is an instruction-fetch stream.
+//     history requested at kernel start): a few hundred KB of straight-line code executed exactly once per call is an
+//     instruction-fetch stream.
 // This kernel keeps the two things that worked (channel groups over warps; every history window of the call requested at
 // kernel start by cp.async.bulk, one mbarrier per layer) and moves the weights back to DATA: ONE bulk copy brings the
 // whole 55 KB blob into shared memory per call (the data path moves it in ~0.6 us; the instruction path needed ~10), and
@@ -459,7 +459,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   {
     // barrier, then ONE system-scope fence by the signalling thread (fences are cumulative: it orders every output store the
     // barrier made it observe before the doorbell -- the grid-sync idiom); a fence by every thread before the barrier as well
-    // only put a second ~2.5 us system fence on the critical path (profiles/r02ze_*: `membar` 1.8 cycles per instruction)
+    // only puts a second system-scope fence on the critical path
     __syncthreads();
     if (tid == 0 && blockIdx.x == 0)
     {

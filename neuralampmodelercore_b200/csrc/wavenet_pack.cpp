@@ -9,8 +9,6 @@ namespace namb200
 
 namespace
 {
-void pack_tc(const ModelSpec& ms, WaveNetPlan& plan);
-
 int pad_channels(int c)
 {
   if (c <= 4)
@@ -33,106 +31,6 @@ int next_pow2(long v)
 size_t align4(size_t n)
 {
   return (n + 3) & ~(size_t)3;
-}
-
-// Round to TF32 (10 explicit mantissa bits), nearest, ties away from zero -- the host twin of
-// cvt.rna.tf32.f32, used to split a weight into hi + lo for the 3xTF32 tensor-core product.
-float tf32_rna(float x)
-{
-  uint32_t u;
-  std::memcpy(&u, &x, 4);
-  if ((u & 0x7F800000u) == 0x7F800000u)
-    return x; // inf / nan
-  u = (u + 0x1000u) & 0xFFFFE000u;
-  float r;
-  std::memcpy(&r, &u, 4);
-  return r;
-}
-
-// Write one B tile: [2 chunks of 4 input channels][16 output channels][4] for K-step `ks` of matrix
-// W (out x in, row-major, `cr` real channels), hi and lo parts.
-void write_b_tile(float* hi, float* lo, const float* w_out_in, int cr_out, int cr_in, int ks)
-{
-  for (int c = 0; c < 2; c++)
-    for (int n = 0; n < 16; n++)
-      for (int i = 0; i < 4; i++)
-      {
-        const int in = 8 * ks + 4 * c + i;
-        float v = 0.0f;
-        if (n < cr_out && in < cr_in)
-          v = w_out_in[(size_t)n * cr_in + in];
-        const float h = tf32_rna(v);
-        hi[(c * 16 + n) * 4 + i] = h;
-        lo[(c * 16 + n) * 4 + i] = v - h;
-      }
-}
-
-// Tensor-core images (layout: wavenet_desc.h).  Eligible when every array is padded to 8 or 16 channels
-// and no layer needs more than 2 staged taps (kernel size 3 with look-back beyond the 64-column halo).
-void pack_tc(const ModelSpec& ms, WaveNetPlan& plan)
-{
-  const WaveNetSpec& wn = ms.wavenet;
-  plan.tc_eligible = false;
-  for (int a = 0; a < plan.n_arrays; a++)
-    if (plan.cp[a] < 8)
-    {
-      plan.tc_why_not = "fewer than 5 channels";
-      return;
-    }
-  for (const ArraySpec& A : wn.arrays)
-    if (A.head_kernel != 1)
-    {
-      plan.tc_why_not = "head kernel size " + std::to_string(A.head_kernel);
-      return;
-    }
-  size_t li = 0;
-  for (size_t a = 0; a < wn.arrays.size(); a++)
-  {
-    const ArraySpec& A = wn.arrays[a];
-    const int cp = plan.cp[a], cr = A.channels;
-    for (const LayerSpec& L : A.layers)
-    {
-      const int K = L.conv.kernel, ks = cp / 8;
-      int staged = 0;
-      for (int k = 0; k < K - 1; k++)
-        if ((K - 1 - k) * L.conv.dilation > kHalo)
-          staged++;
-      plan.tc_max_staged_taps = std::max(plan.tc_max_staged_taps, staged);
-      const int n = tc_image_floats(K, cp);
-      const size_t off = plan.tc_blob.size();
-      plan.tc_blob.resize(off + n, 0.0f);
-      float* img = plan.tc_blob.data() + off;
-      float* conv_hi = img;
-      float* conv_lo = img + (size_t)K * ks * kTcTile;
-      float* p_hi = img + (size_t)2 * K * ks * kTcTile;
-      float* p_lo = p_hi + (size_t)ks * kTcTile;
-      float* vec = p_lo + (size_t)ks * kTcTile;
-      for (int k = 0; k < K; k++)
-        for (int s = 0; s < ks; s++)
-          write_b_tile(conv_hi + ((size_t)k * ks + s) * kTcTile, conv_lo + ((size_t)k * ks + s) * kTcTile,
-                       L.conv.w.data() + (size_t)k * cr * cr, cr, cr, s);
-      for (int s = 0; s < ks; s++)
-        write_b_tile(p_hi + (size_t)s * kTcTile, p_lo + (size_t)s * kTcTile, L.l1x1.w.data(), cr, cr, s);
-      for (int o = 0; o < cr; o++)
-      {
-        vec[o] = L.conv.b[o];
-        vec[16 + o] = L.mixin.w[o];
-        vec[32 + o] = L.l1x1.b[o];
-        if (L.act.type == ActType::PReLU)
-          vec[48 + o] = L.act.slopes.size() == 1 ? L.act.slopes[0] : L.act.slopes[o];
-      }
-      plan.tc_off.push_back((int)off);
-      plan.tc_floats.push_back(n);
-      plan.tc_max_image_floats = std::max(plan.tc_max_image_floats, n);
-      li++;
-    }
-  }
-  if (plan.tc_max_staged_taps > 2)
-  {
-    plan.tc_why_not = "more than 2 taps per layer reach beyond the halo (kernel size > 3 with long dilation)";
-    return;
-  }
-  plan.tc_eligible = true;
 }
 } // namespace
 
@@ -316,7 +214,6 @@ WaveNetPlan plan_wavenet(const ModelSpec& ms)
   plan.head_scale = wn.head_scale;
   plan.macs_per_frame = macs;
   plan.eligible = true;
-  pack_tc(ms, plan);
   return plan;
 }
 

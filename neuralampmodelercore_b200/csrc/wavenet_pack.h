@@ -27,12 +27,6 @@ struct WaveNetPlan
   int max_lookback = 0;
 
   // tensor-core variant
-  bool tc_eligible = false;
-  std::string tc_why_not;
-  std::vector<float> tc_blob;
-  std::vector<int> tc_off, tc_floats;
-  int tc_max_image_floats = 0;
-  int tc_max_staged_taps = 0; // taps per layer whose window is not inside the tile + 64-column halo
 };
 
 /// Decide whether the fused kernel can run this model and, if so, pack it.

@@ -1,12 +1,12 @@
-// wavenet_spec.cuh -- the MODEL-SPECIALISED fused WaveNet kernel for sm_100a.
+// wavenet_spec.cuh -- the MODEL-SPECIALISED fused WaveNet kernel for sm_90a.
 //
 // This file is compiled once per model (NVRTC at load time, jit_spec.cpp; or nvcc for tools/spec_proto.cu) together
 // with a generated header that defines namespace `spec`: the layer table as constexpr data and the weights as
 // `__device__ const unsigned Wb[]` bit patterns read through spec::w(i).  Every loop below has compile-time bounds and is fully unrolled, so every weight
 // becomes the 32-bit IMMEDIATE of an FFMA (`FFMA R, Rx, 0.1234, R`): no weight loads, no weight registers, no
 // shared-memory copy of the weights.  Why: the generic fused kernel (wavenet_fused.cuh) broadcasts weights from shared
-// memory, and at two frames per thread one uniform LDS.128 (2 wavefronts) feeds only 4 FFMA2 -- the shared-memory pipe
-// runs at 67 % while the FMA pipe reaches 59 % (profiles/r01g_*): the two saturate together.  With immediates the FMA
+// memory, and at two frames per thread one uniform LDS.128 (2 wavefronts) feeds only a handful of FMAs per thread -- the
+// shared-memory pipe and the FMA pipe saturate together.  With immediates the FMA
 // pipe is fed by the instruction stream alone; shared memory carries only the activations.
 //
 // What it computes (reference file:line, all under NAM/): the same path as wavenet_fused.cuh --
@@ -84,23 +84,29 @@ __device__ __forceinline__ void unpack2(const u64 v, float& lo, float& hi)
 {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// sm_90 has no packed FP32 arithmetic: a pair operation is two scalar round-to-nearest instructions on the halves (the
+// numbers fma.rn.f32x2 / mul.rn.f32x2 / add.rn.f32x2 give)
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c)
 {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float al, ah, bl, bh, cl, ch;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  unpack2(c, cl, ch);
+  return pack2(__fmaf_rn(al, bl, cl), __fmaf_rn(ah, bh, ch));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b)
 {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float al, ah, bl, bh;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  return pack2(__fmul_rn(al, bl), __fmul_rn(ah, bh));
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b)
 {
-  u64 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float al, ah, bl, bh;
+  unpack2(a, al, ah);
+  unpack2(b, bl, bh);
+  return pack2(__fadd_rn(al, bl), __fadd_rn(ah, bh));
 }
 __device__ __forceinline__ u64 dup2(float v)
 {
@@ -132,12 +138,9 @@ __device__ __forceinline__ float act_sigmoid(float x)
 
 // ---- frame vectors -------------------------------------------------------------------------------------------------------
 // S = 1: a thread owns frame `tid` of ONE stream, V = float.
-// S = 2: a thread owns frame `tid` of a PAIR of streams (2q, 2q + 1), V = a packed f32x2 pair (low half = the even
-// stream).  Everything a layer does is written once over V.  For S = 2 one instruction serves both streams:
-// `FFMA2 Racc, Rx.F32x2, <imm32>, Racc` -- the packed FMA takes the weight as a BROADCAST IMMEDIATE, so the weight stream
-// costs one issue slot and 16 instruction bytes per weight for two frames, and the kernel is bound by the FMA pipe itself
-// instead of by instruction issue / fetch (profiles/r02a_*: S = 1 issues 16,800 instructions per warp-frame, 79 % FFMA,
-// top stall no_instruction).  The pair must sit in an aligned register pair, so the activations of the two streams are
+// S = 2: a thread owns frame `tid` of a PAIR of streams (2q, 2q + 1), V = a register pair (low half = the even
+// stream).  Everything a layer does is written once over V.  The form was made for a packed FMA with a broadcast
+// immediate weight; sm_90 has none, so each pair operation is two scalar FFMAs and S = 1 is the default.  The pair must sit in an aligned register pair, so the activations of the two streams are
 // interleaved element-wise wherever they are stored: a column of a "sub-plane" is 16 bytes = (c A, c B, c' A, c' B) for
 // two channels c, c' -- one LDS.128 yields two ready pairs, conflict-free.  The rings of the library keep one stream
 // per ring ([C/4][R][4 floats]), so the kernel converts a pair's rings into a per-CTA scratch in the interleaved layout
@@ -780,15 +783,15 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
 // The reference's hosts call process() with 64-frame blocks.  With thousands of streams such a step is not latency-bound
 // per stream but occupancy-bound: every stream-call must pull ~61 KB of ring columns (a1_standard, 64 frames) through L2 /
 // HBM, and the precompiled short-call geometry (4 streams per 128-thread CTA, 55 KB of weights in shared memory per CTA)
-// runs 8 warps per SM -- profiles/r02i_short_call_*: long-scoreboard stalls, issue-active 32 %.  Here the weights are
+// runs only 8 warps per SM, too few to hide the ring loads.  Here the weights are
 // immediates, so a CTA is NT / FQ streams side by side (8 x 64 frames at 512 threads), shared memory holds only the
 // tile (32 KB) and 32 warps per SM hide the ring loads.  History is NOT staged: a tap that reaches before the call reads
 // its ring column directly (16 bytes per thread, consecutive frames = consecutive addresses), one that stays inside the
 // call reads the tile.  Same rings as every other kernel.
 //
-// Two things decide this kernel (profiles/r02t_*: a launch is only two passes through ~260 KB of straight-line code, and
-// the 0.5 GB of ring traffic between two launches had pushed that code out of L2, so one pass in two fetched its
-// instructions from HBM -- `no_instruction` 7.3 cycles per issued instruction against 2.1 in the long-call kernel):
+// Two things decide this kernel (a launch is only two passes through a few hundred KB of straight-line code, and the ring
+// traffic between two launches pushes that code out of L2 unless told not to, so that passes fetch their instructions
+// from HBM):
 //  * ring loads / stores carry an L2 evict-first policy, so the code (and nothing else is reused) stays L2-resident;
 //  * each warp prefetches the NEXT layer's ring windows into L2 (one `prefetch.global.L2` per lane) while it computes
 //    this one, so the tap loads meet L2 latency instead of HBM latency.

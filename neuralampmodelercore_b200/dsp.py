@@ -8,7 +8,7 @@ NAM/get_dsp.h:85-116) so the parity tests read like the reference's own tests:
     model.process(inp, out, n)                      # DSP::process(NAM_SAMPLE** in, NAM_SAMPLE** out, n), stream 0
     y = model.process_batch(x)                      # the batched reframing: x[batch, n] float32 -> y[batch, n]
 
-There is no CPU path behind this module: every call goes to libnam_b200.so (hand-written sm_100a
+There is no CPU path behind this module: every call goes to libnam_b200.so (hand-written sm_90a
 kernels) and raises if the library or a CUDA device is missing.
 """
 from __future__ import annotations
@@ -361,7 +361,7 @@ def get_dsp(config, batch: int = 1, device: int = -1, prewarm: Optional[bool] = 
 
 def jit_prepare(config, fast_tanh: Optional[bool] = None, batch: int = 1) -> dict:
     """Host-only: compile (or fetch from the cache) the model-specialised kernel of a WaveNet .nam (path, dict or JSON
-    text).  Needs no GPU: NVRTC cross-compiles for sm_100a.  Returns the library's report as a dict."""
+    text).  Needs no GPU: NVRTC cross-compiles for sm_90a.  Returns the library's report as a dict."""
     import json
 
     lib = _capi.load()
@@ -420,7 +420,7 @@ def submodels(config) -> list:
 
 
 def has_tensor_core_kernel() -> bool:
-    """Was libnam_b200.so built with the tcgen05 / TMEM WaveNet kernel (NAM_B200_BUILD_TC=1; kernel_geometry=3)?"""
+    """Does libnam_b200.so have a tensor-core WaveNet kernel (kernel_geometry=3)?  Never on sm_90a."""
     return bool(_capi.load().nam_b200_has_tensor_core_kernel())
 
 

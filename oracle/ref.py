@@ -36,7 +36,7 @@ def build(force: bool = False) -> bool:
     """Compile the reference where its sources are mounted; returns False (and builds nothing) elsewhere."""
     if not (REFERENCE_TREE / "NAM" / "dsp.cpp").exists():
         return False
-    cmd = ["make", "-C", str(HERE), "ref"] + (["-B"] if force else [])
+    cmd = ["make", "-C", str(HERE), "ref", "ref-tools"] + (["-B"] if force else [])
     subprocess.run(cmd, check=True, capture_output=True)
     return True
 

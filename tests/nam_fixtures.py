@@ -1,8 +1,9 @@
 """Test helpers: committed model fixtures (tests/golden/models/*.npz), the decoded example input and
-the synthetic benchmark signal of SURVEY.md section 8(d).  Nothing here reads /root/reference."""
+the synthetic benchmark signal of SURVEY.md section 8(d).  Nothing here reads the reference's source tree."""
 from __future__ import annotations
 
 import json
+import os
 from pathlib import Path
 
 import numpy as np
@@ -41,6 +42,34 @@ def oracle_golden(name: str, regime: str) -> dict:
 
 def decimate(y: np.ndarray) -> dict:
     return {"head": y[:512], "transition": y[46000:50096], "strided": y[::37]}
+
+
+REFERENCE_OUTPUTS = GOLDEN / "reference_outputs.npz"
+
+
+def sample(y: np.ndarray) -> np.ndarray:
+    """The part of an output (time on the last axis) that tests/golden/reference_outputs.npz keeps: all of it up to
+    1024 frames, else the first 128 frames and every 16th frame after them."""
+    y = np.asarray(y, dtype=np.float32)
+    n = y.shape[-1]
+    return y if n <= 1024 else y[..., np.r_[0:128, 128:n:16]]
+
+
+def reference(key: str, compute) -> np.ndarray:
+    """What the reference (NeuralAmpModelerCore itself, oracle/_ref) computes for the test case `key`, sampled as by
+    `sample()`, from tests/golden/reference_outputs.npz.  `compute` is the case's recipe against the reference build
+    (oracle.ref): with NAM_REFERENCE_RECORD=1, where oracle/_ref is built, it runs and its result replaces the stored one."""
+    if os.environ.get("NAM_REFERENCE_RECORD") == "1":
+        y = sample(compute())
+        store = {}
+        if REFERENCE_OUTPUTS.exists():
+            with np.load(REFERENCE_OUTPUTS) as z:
+                store = {k: z[k] for k in z.files}
+        store[key] = y
+        np.savez_compressed(REFERENCE_OUTPUTS, **store)
+        return y
+    with np.load(REFERENCE_OUTPUTS) as z:
+        return z[key]
 
 
 def synthetic_batch(batch: int, n: int, seed: int = 1234, rate: float = 48000.0) -> np.ndarray:

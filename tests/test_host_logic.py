@@ -289,22 +289,3 @@ def test_jit_compiles_without_a_gpu_and_the_sass_is_what_design_md_says(tmp_path
             "weights": [0.01 * i for i in range(4 * 3 * 4 + 4 * 3 + 6 + 3 + 1)], "sample_rate": 48000}
     assert nb.jit_prepare(lstm, fast_tanh=True)["ok"]
     assert nb.jit_prepare(fx.load_model("wavenet_a2_max"), fast_tanh=False)["ok"]
-
-
-def test_tensor_core_kernel_is_a_build_option(monkeypatch):
-    """NAM_B200_BUILD_TC selects the object of csrc/wavenet_tc_launch.cu (kernel or stubs); the option a library was linked
-    with is recorded next to it, and the library reports it (no GPU needed)."""
-    from neuralampmodelercore_b200 import _build
-
-    monkeypatch.delenv("NAM_B200_BUILD_TC", raising=False)
-    assert not _build.with_tc()
-    assert _build._obj_name(_build.CSRC / "wavenet_tc_launch.cu") == "wavenet_tc_launch.cu.o"
-    monkeypatch.setenv("NAM_B200_BUILD_TC", "1")
-    assert _build.with_tc()
-    assert _build._obj_name(_build.CSRC / "wavenet_tc_launch.cu") == "wavenet_tc_launch.cu.tc1.o"
-    assert _build._obj_name(_build.CSRC / "nam_b200.cu") == "nam_b200.cu.o"  # only that one object depends on the option
-    assert _build._options_stamp() == "tc=1\n"
-    monkeypatch.delenv("NAM_B200_BUILD_TC")
-    stamp = (_build.LIB_DIR / "build_options.txt").read_text()
-    assert stamp in ("tc=0\n", "tc=1\n")
-    assert nb.has_tensor_core_kernel() == (stamp == "tc=1\n")

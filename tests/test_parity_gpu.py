@@ -3,7 +3,7 @@ oracle on the same inputs.  Tolerance: 1e-5 max-abs in float32 (BASELINE.json no
 regimes.  Protocols follow the reference's tools: render.cpp (Reset(sr, 64) + 64-frame blocks on
 example_audio/input.wav) and test_a2_fast.cpp (seeded weights, two-tone input, several block sizes).
 
-Run with `pytest -m gpu` on the B200 box.
+Run with `pytest -m gpu` on an H100.
 """
 import numpy as np
 import pytest
@@ -320,7 +320,7 @@ def test_pipelined_host_call_equals_the_single_launch():
     import torch
 
     nam = fx.load_model("wavenet_a1_standard")
-    B, n = 2700, 1024  # 10.5 MiB per direction: three chunks of 1184 / 1184 / 332 streams on a 148-SM part
+    B, n = 2700, 1024  # 10.5 MiB per direction: three chunks of 1056 / 1056 / 588 streams on a 132-SM part
     x = fx.synthetic_batch(B, 2 * n, seed=77)
     a = nb.get_dsp(nam, batch=B, fast_tanh=True)
     b = nb.get_dsp(nam, batch=B, fast_tanh=True)

@@ -1,9 +1,10 @@
-// microbench.cu -- design-constant measurements for the fused WaveNet kernel (sm_100a).
-//   1. FP32 FMA issue rate: scalar FFMA vs packed FFMA2, by resident warps per SM
+// microbench.cu -- design-constant measurements for the fused WaveNet kernel (sm_90a).
+//   1. FP32 FFMA issue rate by resident warps per SM
 //   2. the kernel's inner-loop pattern: one warp-uniform weight row (16 floats = 4 x LDS.128)
-//      feeding S x 8 FFMA2 (S = time steps per thread); weights from shared memory or from
+//      feeding S x 8 pair FMAs (S = time steps per thread); weights from shared memory or from
 //      __constant__ memory
-// Prints one JSON object per line.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench microbench.cu
+// sm_90 has no packed FP32 FMA, so a pair FMA is two scalar FFMAs (ffma2 below).
+// Prints one JSON object per line.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench microbench.cu
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -21,7 +22,11 @@
     }                                                                                                                \
   } while (0)
 
-template <bool PACKED>
+__device__ __forceinline__ float2 ffma2(const float2 a, const float2 b, const float2 c)
+{
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
 __global__ void fma_peak(float* out, int iters, float seed)
 {
   float2 a[8];
@@ -35,13 +40,8 @@ __global__ void fma_peak(float* out, int iters, float seed)
 #pragma unroll
     for (int i = 0; i < 8; i++)
     {
-      if (PACKED)
-        a[i] = __ffma2_rn(a[i], m, c);
-      else
-      {
-        a[i].x = fmaf(a[i].x, m.x, c.x);
-        a[i].y = fmaf(a[i].y, m.y, c.y);
-      }
+      a[i].x = fmaf(a[i].x, m.x, c.x);
+      a[i].y = fmaf(a[i].y, m.y, c.y);
     }
   }
   float s = 0.0f;
@@ -107,8 +107,8 @@ __global__ void __launch_bounds__(128) inner_loop(const float4* __restrict__ w, 
 #pragma unroll
         for (int q = 0; q < 4; q++)
         {
-          acc[j][2 * q] = __ffma2_rn(make_float2(wq[q].x, wq[q].y), xx, acc[j][2 * q]);
-          acc[j][2 * q + 1] = __ffma2_rn(make_float2(wq[q].z, wq[q].w), xx, acc[j][2 * q + 1]);
+          acc[j][2 * q] = ffma2(make_float2(wq[q].x, wq[q].y), xx, acc[j][2 * q]);
+          acc[j][2 * q + 1] = ffma2(make_float2(wq[q].z, wq[q].w), xx, acc[j][2 * q + 1]);
         }
         x[j] += 1e-6f;
       }
@@ -147,25 +147,21 @@ int main()
   CK(cudaEventCreate(&e1));
 
   // 1. raw FMA peaks vs resident warps per SM
-  for (int packed = 0; packed < 2; packed++)
-    for (int warps_per_sm : {4, 8, 16, 32, 64})
+  for (int warps_per_sm : {4, 8, 16, 32, 64})
+  {
+    const int threads = 128, blocks = sms * (warps_per_sm / 4), iters = 8192;
+    double best = 1e30;
+    for (int rep = 0; rep < 4; rep++)
     {
-      const int threads = 128, blocks = sms * (warps_per_sm / 4), iters = 8192;
-      double best = 1e30;
-      for (int rep = 0; rep < 4; rep++)
-      {
-        CK(cudaEventRecord(e0));
-        if (packed)
-          fma_peak<true><<<blocks, threads>>>(d, iters, 1.f);
-        else
-          fma_peak<false><<<blocks, threads>>>(d, iters, 1.f);
-        CK(cudaEventRecord(e1));
-        best = fmin(best, time_ms(e0, e1));
-      }
-      const double fma = 16.0 * iters * (double)blocks * threads;
-      printf("{\"test\": \"fma_peak\", \"packed\": %d, \"warps_per_sm\": %d, \"tflops\": %.2f, \"fma_per_clk_per_sm_at_max_clock\": %.1f}\n",
-             packed, warps_per_sm, 2 * fma / (best * 1e-3) / 1e12, fma / (best * 1e-3) / sms / (clock_khz * 1e3));
+      CK(cudaEventRecord(e0));
+      fma_peak<<<blocks, threads>>>(d, iters, 1.f);
+      CK(cudaEventRecord(e1));
+      best = fmin(best, time_ms(e0, e1));
     }
+    const double fma = 16.0 * iters * (double)blocks * threads;
+    printf("{\"test\": \"fma_peak\", \"warps_per_sm\": %d, \"tflops\": %.2f, \"fma_per_clk_per_sm_at_max_clock\": %.1f}\n",
+           warps_per_sm, 2 * fma / (best * 1e-3) / 1e12, fma / (best * 1e-3) / sms / (clock_khz * 1e3));
+  }
 
   // 2. inner loop pattern
   std::vector<float4> hw(kRows * 4);

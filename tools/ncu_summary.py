@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an Nsight Compute report (.ncu-rep, read here without a GPU) into the small, tracked files
-under profiles/: a JSON of the headline metrics of the dominant kernel plus an opcode / phase breakdown
-from the source page.  Usage: python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r01_fused_kernel"""
+"""Summarise an Nsight Compute report (.ncu-rep, read without a GPU) into small files: a JSON of the headline
+metrics of the dominant kernel plus an opcode / phase breakdown from the source page.
+Usage: python tools/ncu_summary.py <report>.ncu-rep <output prefix>"""
 from __future__ import annotations
 
 import collections
@@ -82,7 +82,7 @@ def main() -> None:
     summary["phases_between_barriers"] = [
         {"instructions_share": round(p["instructions"] / tot, 4), "sample_share": round(p["samples"] / tots, 4),
          "ffma2_share_of_phase": round(p["ffma2"] / max(p["instructions"], 1), 3)} for p in phases if p["instructions"] > tot * 0.002][:48]
-    # ("ffma2" counts FFMA2 and scalar FFMA: the model-specialised kernel issues its weights as FFMA immediates)
+    # ("ffma2" counts packed FFMA2, where the architecture has it, and scalar FFMA)
     summary["top_stall_instructions"] = [{"sample_share": round(sp / tots, 4), "executed": n, "sass": t}
                                          for sp, n, t in sorted(hot, reverse=True)[:24]]
     with open(out_prefix + ".json", "w") as f:

@@ -1,5 +1,5 @@
 // spec_proto.cu -- stand-alone timing of the model-specialised kernel (wavenet_spec.cuh) on a generated model header.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -I<dir of spec_model.h> -o spec_proto spec_proto.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -I<dir of spec_model.h> -o spec_proto spec_proto.cu
 #include <cuda_runtime.h>
 
 #include <cstdio>
