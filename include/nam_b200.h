@@ -118,6 +118,52 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames);
 /* DSP::prewarm() on its own (after a reset with prewarm_on_reset == 0). */
 int nam_b200_prewarm(nam_b200_model* m);
 
+/* ---- per-stream state: reset, copy, export and import single streams ----------------------------------------------
+ * A stream's state travels as a RECORD that does not depend on the handle's kernel, geometry or max_batch: a 64-byte
+ * header -- magic "NAMS", uint32 format version 1, uint32 architecture (as nam_b200_info), uint32 0, uint64 payload float
+ * count, uint64 model fingerprint (a hash of the architecture, the parsed config and the weight bits; fast_tanh and the
+ * handle options are not part of it), zeros -- then the float32 payload, little-endian:
+ *   WaveNet / ConvNet: per convolution with a look-back (K-1)*d > 0, in weight-stream order (the main network's layer
+ *     convolutions and head convolutions, then a condition_dsp sub-model's), the last look-back columns of its input,
+ *     oldest first, each column the real channel count;  LSTM: per layer h[H] then c[H];  Linear: the last
+ *     receptive_field - 1 input samples, oldest first.
+ * nam_b200_state_layout_json lists the segments.  A record can be stored per user session, moved to another handle of the
+ * same model (any options) or to another GPU.  SlimmableContainer handles act on the active sub-model, whose fingerprint a
+ * record carries: a record taken at one slimmable size is refused at another.
+ *
+ * The handle keeps, per stream, the clock value at which the stream's history ends.  A stream left out of process calls
+ * (batch < max_batch) keeps its history at that older point: export reads it there, correctly; but process_* reads every
+ * stream at the handle's current clock, so such a stream must be brought back with export + import, or with
+ * nam_b200_reset_streams, before it takes part in a call again.
+ *
+ * Stream lists hold indices in [0, max_batch); destinations must be distinct.  Everything is checked on the host before
+ * anything runs (NAM_B200_ERR_INVALID_ARGUMENT with the offending stream and field; NAM_B200_ERR_STATE before reset). */
+
+/* Bytes of one record (header + payload). */
+int64_t nam_b200_stream_state_size(const nam_b200_model* m);
+/* DSP::Reset for the listed streams only, with the last reset's settings (prewarm_on_reset, max_frames); every other stream is
+ * untouched.  WaveNet / ConvNet / Linear: the state nam_b200_reset leaves (fresh is ignored).  LSTM: fresh = 0 keeps h, c and
+ * prewarms on top of them, as nam_b200_reset does; fresh = 1 starts from the trained h0, c0 like a newly created handle. */
+int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int fresh);
+/* dst[i] takes src[i]'s state (all sources are read before any destination is written: a swap works). */
+int nam_b200_copy_streams(nam_b200_model* m, const int32_t* src, const int32_t* dst, int n);
+/* Record of streams[i] -> dst + i * record_stride (record_stride >= nam_b200_stream_state_size).  Host memory, staged
+ * through the device on the handle's stream; returns when the records are in `dst`. */
+int nam_b200_export_streams(nam_b200_model* m, const int32_t* streams, int n, void* dst, int64_t record_stride);
+/* Records src + i * record_stride -> streams[i] (whose histories then end at the handle's clock).  Host memory; every
+ * header is checked before anything is copied; returns when done. */
+int nam_b200_import_streams(nam_b200_model* m, const int32_t* streams, int n, const void* src, int64_t record_stride);
+/* The same on device memory (4-byte aligned records), asynchronous on `cuda_stream` (NULL = the handle's stream).  The import
+ * first copies the n headers (64 B each) to the host and checks them, synchronising `cuda_stream` once, before it launches. */
+int nam_b200_export_streams_device(nam_b200_model* m, const int32_t* streams, int n, void* dst_device, int64_t record_stride,
+                                   void* cuda_stream);
+int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, int n, const void* src_device,
+                                   int64_t record_stride, void* cuda_stream);
+/* Host-only, no CUDA: the record of a .nam document as a JSON object -- architecture, header_bytes, payload_floats,
+ * record_bytes, fingerprint, segments [{name, channels, columns, offset (floats into the payload)}].  A SlimmableContainer
+ * describes its default (largest) sub-model.  Returns 0, or the error codes of create. */
+int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t capacity);
+
 /* Batched throughput entry: `batch` (<= max_batch) streams, stream b reads
  * in[b*in_stride .. +n_frames) and writes out[b*out_stride .. +n_frames); n_frames <= max_frames.
  * Multi-channel models (in_channels / out_channels of nam_b200_info != 1; WaveNet: NAM/wavenet/model.cpp:809-820,

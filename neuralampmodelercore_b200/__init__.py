@@ -17,6 +17,7 @@ from .dsp import (  # noqa: F401
     jit_prepare,
     measure_fp32_tflops,
     has_tensor_core_kernel,
+    state_layout,
     submodels,
     using_fast_tanh,
 )
@@ -29,6 +30,7 @@ __all__ = [
     "inspect",
     "jit_prepare",
     "submodels",
+    "state_layout",
     "enable_fast_tanh",
     "disable_fast_tanh",
     "using_fast_tanh",

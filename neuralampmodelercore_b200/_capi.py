@@ -93,6 +93,14 @@ EXPORTED_SYMBOLS = [
     "nam_b200_multi_shard",
     "nam_b200_multi_reset",
     "nam_b200_multi_process_f32",
+    "nam_b200_stream_state_size",
+    "nam_b200_reset_streams",
+    "nam_b200_copy_streams",
+    "nam_b200_export_streams",
+    "nam_b200_import_streams",
+    "nam_b200_export_streams_device",
+    "nam_b200_import_streams_device",
+    "nam_b200_state_layout_json",
 ]
 
 
@@ -167,6 +175,19 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_measure_fp32_tflops.restype = C.c_double
     lib.nam_b200_has_tensor_core_kernel.argtypes = []
     lib.nam_b200_has_tensor_core_kernel.restype = C.c_int
+    i32p = C.POINTER(C.c_int32)
+    lib.nam_b200_stream_state_size.argtypes = [vp]
+    lib.nam_b200_stream_state_size.restype = C.c_int64
+    lib.nam_b200_reset_streams.argtypes = [vp, i32p, C.c_int, C.c_int]
+    lib.nam_b200_copy_streams.argtypes = [vp, i32p, i32p, C.c_int]
+    lib.nam_b200_export_streams.argtypes = [vp, i32p, C.c_int, vp, C.c_int64]
+    lib.nam_b200_import_streams.argtypes = [vp, i32p, C.c_int, vp, C.c_int64]
+    lib.nam_b200_export_streams_device.argtypes = [vp, i32p, C.c_int, vp, C.c_int64, vp]
+    lib.nam_b200_import_streams_device.argtypes = [vp, i32p, C.c_int, vp, C.c_int64, vp]
+    lib.nam_b200_state_layout_json.argtypes = [C.c_char_p, C.c_char_p, C.c_int64]
+    for name in ("nam_b200_reset_streams", "nam_b200_copy_streams", "nam_b200_export_streams", "nam_b200_import_streams",
+                 "nam_b200_export_streams_device", "nam_b200_import_streams_device", "nam_b200_state_layout_json"):
+        getattr(lib, name).restype = C.c_int
     for name in (
         "nam_b200_create_from_file",
         "nam_b200_create_from_json",

@@ -24,6 +24,7 @@
 #include "generic_pack.h"
 #include "wavenet_generic.cuh"
 #include "jit_spec.h"
+#include "stream_state.cuh"
 
 using namespace namb200;
 
@@ -419,6 +420,22 @@ struct nam_b200_model
   float* d_state = nullptr;
   float* d_state_tmp = nullptr; // Linear double buffer
   long state_stride = 0; // floats
+  // per-stream state control (stream_state.cuh)
+  std::vector<uint32_t> stream_clock; // t_base at which each stream's history ends (streams left out of calls fall behind)
+  std::vector<uint32_t> stream_flips; // Linear: lin_flips when the stream's history was written (parity picks the buffer)
+  uint32_t lin_flips = 0; // Linear: d_state / d_state_tmp swaps so far
+  std::vector<StateSegDesc> state_descs; // record segments -> device layout, built at creation
+  std::vector<StateChunk> state_chunks;
+  StateSegDesc* d_state_descs = nullptr;
+  StateChunk* d_state_chunks = nullptr;
+  long record_floats = 0; // payload floats of one record
+  StateRecordHeader record_header{};
+  std::string state_error; // non-empty: the stream-state calls are refused with this reason
+  unsigned char* d_fresh = nullptr; // WaveNet / ConvNet / Linear: the record of a stream straight after nam_b200_reset
+  StreamRef* d_refs = nullptr; // stream lists of pack / unpack / row-copy launches
+  size_t refs_capacity = 0;
+  unsigned char* d_xfer = nullptr; // staging of host records, scratch rows of copies and LSTM prewarms
+  size_t xfer_bytes = 0;
   // staging
   float* d_in = nullptr;
   float* d_out = nullptr;
@@ -459,6 +476,16 @@ struct nam_b200_model
       cudaFree(d_state);
     if (d_state_tmp)
       cudaFree(d_state_tmp);
+    if (d_state_descs)
+      cudaFree(d_state_descs);
+    if (d_state_chunks)
+      cudaFree(d_state_chunks);
+    if (d_fresh)
+      cudaFree(d_fresh);
+    if (d_refs)
+      cudaFree(d_refs);
+    if (d_xfer)
+      cudaFree(d_xfer);
     if (d_in)
       cudaFree(d_in);
     if (d_out)
@@ -1371,12 +1398,16 @@ void setup_generic_spec_kernel(nam_b200_model* m)
   m->spec_note = std::string("general kernel, ") + (b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s");
 }
 
+// `state`: rows of per-stream state to run on (nullptr = the handle's d_state; nam_b200_reset_streams prewarms a gathered
+// subset of streams in scratch rows)
 void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                 long out_stride, cudaStream_t st)
+                 long out_stride, cudaStream_t st, float* state = nullptr)
 {
+  if (!state)
+    state = m->d_state;
   if (m->spec_state == 1)
   {
-    LstmSpecKernelParams sp{m->d_state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames};
+    LstmSpecKernelParams sp{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames};
     void* args[] = {&sp};
     // The step rate is bound by one warp's instruction stream as long as every warp has a scheduler to itself: four
     // lanes per stream (gate-split, 8 streams per warp: a shorter dependent chain per step) while every warp still gets a
@@ -1397,7 +1428,7 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   LstmKernelParams kp{};
   kp.weights = m->d_weights;
   kp.n_weight_floats = (int)m->n_weight_floats;
-  kp.state = m->d_state;
+  kp.state = state;
   kp.state_stride = (int)m->state_stride;
   kp.in = d_in;
   kp.out = d_out;
@@ -1489,6 +1520,10 @@ void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch
     CUDA_CHECK(cudaGetLastError());
     m->launches++;
     std::swap(m->d_state, m->d_state_tmp);
+    // streams [batch, max_batch) keep their history in the buffer they were last written to
+    m->lin_flips++;
+    for (int b = 0; b < batch; b++)
+      m->stream_flips[(size_t)b] = m->lin_flips;
   }
 }
 
@@ -1546,7 +1581,17 @@ void run_device(nam_b200_model* m, const float* d_in, float* d_out, int batch, i
     default: throw std::runtime_error("no kernel for this architecture");
   }
   m->t_base += (uint32_t)n_frames;
+  uint32_t* clock = m->stream_clock.data();
+  for (int b = 0; b < batch; b++)
+    clock[b] = m->t_base;
   m->streams_identical = false; // (prewarm() restores the flag: it feeds every stream the same zeros)
+}
+
+// every stream's history ends at the handle's clock (init_state, prewarm)
+void set_all_clocks(nam_b200_model* m)
+{
+  std::fill(m->stream_clock.begin(), m->stream_clock.end(), m->t_base);
+  std::fill(m->stream_flips.begin(), m->stream_flips.end(), m->lin_flips);
 }
 
 void ensure_staging(nam_b200_model* m, size_t floats)
@@ -1602,6 +1647,7 @@ void init_state(nam_b200_model* m)
   if (m->spec.arch == Arch::Linear && m->d_state_tmp)
     CUDA_CHECK(cudaMemsetAsync(m->d_state_tmp, 0, total * sizeof(float), m->stream));
   m->t_base = 0;
+  set_all_clocks(m);
   m->streams_identical = true;
   m->state_initialised = true;
 }
@@ -1647,7 +1693,180 @@ void prewarm(nam_b200_model* m)
   if (m->spec.arch == Arch::Linear && m->d_state_tmp)
     CUDA_CHECK(cudaMemcpyAsync(m->d_state_tmp, m->d_state, (size_t)m->state_stride * m->opts.max_batch * sizeof(float),
                                cudaMemcpyDeviceToDevice, m->stream));
+  set_all_clocks(m); // (broadcast or not, every stream now ends where stream 0 does)
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
+}
+
+// ---- per-stream state records (stream_state.h / .cuh) ------------------------------------------------------------------
+// The handle's descriptor table, built once at creation.  A layout the record cannot describe (an internal mismatch) leaves
+// the handle working and only the stream-state calls refused, with the reason (nam_b200_model::state_error).
+size_t record_bytes(const nam_b200_model* m)
+{
+  return (size_t)kStateHeaderBytes + 4 * (size_t)m->record_floats;
+}
+
+void setup_state_records(nam_b200_model* m)
+{
+  const bool gen = (m->spec.arch == Arch::WaveNet && m->use_generic) || m->spec.arch == Arch::ConvNet;
+  const bool fused = m->spec.arch == Arch::WaveNet && !m->use_generic;
+  m->state_descs = state_descs(m->spec, fused ? &m->plan : nullptr, gen ? &m->gplan : nullptr);
+  m->record_floats = 0;
+  for (const StateSegDesc& d : m->state_descs)
+    m->record_floats += (long)d.lookback * d.cr;
+  if (m->state_descs.empty()) // (a model without history: launches still write the record headers)
+    m->state_descs.push_back(StateSegDesc{kSegFlat, 0, 1, 1, 0, 0, 0, 0});
+  m->state_chunks = state_chunks(m->state_descs);
+  if (m->state_chunks.empty())
+    m->state_chunks.push_back(StateChunk{0, 0});
+  m->record_header = state_record_header(m->spec, m->record_floats);
+  CUDA_CHECK(cudaMalloc(&m->d_state_descs, m->state_descs.size() * sizeof(StateSegDesc)));
+  CUDA_CHECK(cudaMemcpy(m->d_state_descs, m->state_descs.data(), m->state_descs.size() * sizeof(StateSegDesc), cudaMemcpyHostToDevice));
+  CUDA_CHECK(cudaMalloc(&m->d_state_chunks, m->state_chunks.size() * sizeof(StateChunk)));
+  CUDA_CHECK(cudaMemcpy(m->d_state_chunks, m->state_chunks.data(), m->state_chunks.size() * sizeof(StateChunk), cudaMemcpyHostToDevice));
+  CUDA_CHECK(cudaMalloc(&m->d_fresh, record_bytes(m)));
+}
+
+void ensure_xfer(nam_b200_model* m, size_t bytes)
+{
+  if (bytes <= m->xfer_bytes)
+    return;
+  if (m->d_xfer)
+    cudaFree(m->d_xfer);
+  m->d_xfer = nullptr;
+  m->xfer_bytes = 0;
+  CUDA_CHECK(cudaMalloc(&m->d_xfer, bytes));
+  m->xfer_bytes = bytes;
+}
+
+// stream list -> device (d_refs); ordered on `st` before the launch that reads it
+const StreamRef* upload_refs(nam_b200_model* m, const std::vector<StreamRef>& refs, cudaStream_t st)
+{
+  if (refs.size() > m->refs_capacity)
+  {
+    if (m->d_refs)
+      cudaFree(m->d_refs);
+    m->d_refs = nullptr;
+    m->refs_capacity = 0;
+    CUDA_CHECK(cudaMalloc(&m->d_refs, refs.size() * sizeof(StreamRef)));
+    m->refs_capacity = refs.size();
+  }
+  CUDA_CHECK(cudaMemcpyAsync(m->d_refs, refs.data(), refs.size() * sizeof(StreamRef), cudaMemcpyHostToDevice, st));
+  return m->d_refs;
+}
+
+dim3 state_grid(const nam_b200_model* m, int n)
+{
+  return dim3((unsigned)m->state_chunks.size(), (unsigned)std::min(n, 65535));
+}
+
+// pack streams[0..n) at their own clocks into records dst + i * stride
+void export_records(nam_b200_model* m, const int32_t* streams, int n, unsigned char* dst, long stride, cudaStream_t st)
+{
+  std::vector<StreamRef> refs((size_t)n);
+  const bool linear = m->spec.arch == Arch::Linear;
+  for (int i = 0; i < n; i++)
+  {
+    const size_t s = (size_t)streams[i];
+    refs[(size_t)i] = StreamRef{streams[i], m->stream_clock[s], (linear && ((m->lin_flips - m->stream_flips[s]) & 1u)) ? 1 : 0, 0};
+  }
+  StatePackParams p{};
+  p.segs = m->d_state_descs;
+  p.chunks = m->d_state_chunks;
+  p.state = m->d_state;
+  p.state_alt = m->d_state_tmp ? m->d_state_tmp : m->d_state;
+  p.state_stride = m->state_stride;
+  p.refs = upload_refs(m, refs, st);
+  p.n = n;
+  p.rec = dst;
+  p.rec_stride = stride;
+  std::memcpy(p.header, &m->record_header, sizeof p.header);
+  state_pack_kernel<<<state_grid(m, n), kStateThreads, 0, st>>>(p);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+}
+
+// the streams' histories now end at the handle's clock, in the buffer the next call reads
+void mark_written(nam_b200_model* m, const int32_t* streams, int n)
+{
+  for (int i = 0; i < n; i++)
+  {
+    m->stream_clock[(size_t)streams[i]] = m->t_base;
+    m->stream_flips[(size_t)streams[i]] = m->lin_flips;
+  }
+  m->streams_identical = false; // (a later prewarm must not broadcast stream 0 over them)
+}
+
+// unpack records src + i * stride (stride 0: one record for all) into streams[0..n) at the handle's clock
+void import_records(nam_b200_model* m, const int32_t* streams, int n, const unsigned char* src, long stride, cudaStream_t st)
+{
+  std::vector<StreamRef> refs((size_t)n);
+  for (int i = 0; i < n; i++)
+    refs[(size_t)i] = StreamRef{streams[i], m->t_base, 0, 0};
+  StateUnpackParams p{};
+  p.segs = m->d_state_descs;
+  p.chunks = m->d_state_chunks;
+  p.state = m->d_state;
+  p.state_stride = m->state_stride;
+  p.refs = upload_refs(m, refs, st);
+  p.n = n;
+  p.rec = src;
+  p.rec_stride = stride;
+  state_unpack_kernel<<<state_grid(m, n), kStateThreads, 0, st>>>(p);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+  mark_written(m, streams, n);
+}
+
+// whole state rows: dst[dst_refs[i].stream or i] = src[src_refs[i].stream or i]
+void copy_rows(nam_b200_model* m, float* dst, const StreamRef* dst_refs, const float* src, const StreamRef* src_refs, int n,
+               cudaStream_t st)
+{
+  const long stride4 = m->state_stride / 4;
+  const dim3 grid((unsigned)((stride4 + kStateThreads - 1) / kStateThreads), (unsigned)std::min(n, 65535));
+  state_rows_kernel<<<grid, kStateThreads, 0, st>>>(reinterpret_cast<float4*>(dst), reinterpret_cast<const float4*>(src), stride4,
+                                                      dst_refs, src_refs, n);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+}
+
+// nam_b200_reset for an LSTM keeps h, c and prewarms on top (fresh: from h0 / c0, like a new handle): the listed streams'
+// rows are gathered into scratch, prewarmed there exactly like prewarm() (zeros in max_frames blocks), scattered back
+void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fresh)
+{
+  const size_t row = (size_t)m->state_stride;
+  ensure_xfer(m, (size_t)n * row * sizeof(float));
+  float* rows = reinterpret_cast<float*>(m->d_xfer);
+  std::vector<StreamRef> refs((size_t)n);
+  for (int i = 0; i < n; i++)
+    refs[(size_t)i] = StreamRef{streams[i], m->t_base, 0, 0};
+  const StreamRef* d_refs = upload_refs(m, refs, m->stream);
+  if (fresh)
+  {
+    std::vector<float> h((size_t)n * row, 0.0f);
+    const int H = m->spec.lstm.hidden;
+    for (int i = 0; i < n; i++)
+      for (int l = 0; l < m->spec.lstm.num_layers; l++)
+      {
+        float* r = h.data() + (size_t)i * row + (size_t)l * 2 * H;
+        std::copy(m->spec.lstm.cells[l].h0.begin(), m->spec.lstm.cells[l].h0.end(), r);
+        std::copy(m->spec.lstm.cells[l].c0.begin(), m->spec.lstm.cells[l].c0.end(), r + H);
+      }
+    CUDA_CHECK(cudaMemcpyAsync(rows, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+  }
+  else
+    copy_rows(m, rows, nullptr, m->d_state, d_refs, n, m->stream);
+  const int ps = m->spec.prewarm_samples;
+  if (m->opts.prewarm_on_reset && ps > 0)
+  {
+    const int bs = std::max(m->max_frames, 1);
+    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
+    ensure_staging(m, (size_t)n * bs * std::max(ci, co));
+    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
+    for (int done = 0; done < ps; done += bs)
+      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, rows);
+  }
+  copy_rows(m, m->d_state, d_refs, rows, nullptr, n, m->stream);
+  mark_written(m, streams, n);
 }
 
 int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_model** out)
@@ -1830,6 +2049,20 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
     CUDA_CHECK(cudaMalloc(&m->d_state, std::max<size_t>(state_total, 4) * sizeof(float)));
     if (m->spec.arch == Arch::Linear)
       CUDA_CHECK(cudaMalloc(&m->d_state_tmp, std::max<size_t>(state_total, 4) * sizeof(float)));
+    m->stream_clock.assign((size_t)m->opts.max_batch, 0u);
+    m->stream_flips.assign((size_t)m->opts.max_batch, 0u);
+    try
+    {
+      setup_state_records(m.get());
+    }
+    catch (const CudaError&)
+    {
+      throw;
+    }
+    catch (const std::exception& ex)
+    {
+      m->state_error = ex.what();
+    }
     init_state(m.get());
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
   }
@@ -1961,6 +2194,78 @@ int process_planar(nam_b200_model* m, const T* const* input, T* const* output, i
     return NAM_B200_OK;
   });
 }
+
+// ---- argument checks of the stream-state calls: all on the host, before anything is launched ---------------------------
+int check_state_calls(nam_b200_model* m, const char* fn)
+{
+  if (!m->state_error.empty())
+    return fail(NAM_B200_ERR_UNSUPPORTED, std::string(fn) + ": no per-stream state records for this handle: " + m->state_error);
+  if (!m->is_reset)
+    return fail(NAM_B200_ERR_STATE, std::string(fn) + " called before reset");
+  return NAM_B200_OK;
+}
+
+int check_stream_list(const nam_b200_model* m, const int32_t* idx, int n, const char* what, bool distinct)
+{
+  if (n < 0)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, std::string(what) + ": negative stream count " + std::to_string(n));
+  if (n > 0 && !idx)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, std::string(what) + ": null stream list");
+  std::vector<char> seen(distinct ? (size_t)m->opts.max_batch : 0, 0);
+  for (int i = 0; i < n; i++)
+  {
+    const int32_t s = idx[i];
+    const std::string at = std::string(what) + "[" + std::to_string(i) + "] = " + std::to_string(s);
+    if (s < 0 || s >= m->opts.max_batch)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + ": stream index outside [0, max_batch=" + std::to_string(m->opts.max_batch) + ")");
+    if (distinct && seen[(size_t)s]++)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + ": duplicate destination stream");
+  }
+  return NAM_B200_OK;
+}
+
+int check_records(const nam_b200_model* m, const void* buf, int n, int64_t stride, bool device)
+{
+  if (n > 0 && !buf)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null record buffer");
+  const size_t rb = record_bytes(m);
+  if (stride < (int64_t)rb)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "record_stride " + std::to_string(stride) + " is smaller than the record ("
+                                                 + std::to_string(rb) + " bytes)");
+  if (device && (stride % 4 != 0 || reinterpret_cast<uintptr_t>(buf) % 4 != 0))
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "device records must be 4-byte aligned (record_stride " + std::to_string(stride) + ")");
+  return NAM_B200_OK;
+}
+
+// the header of record i (for stream `stream`) must be this model's
+int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i, int stream)
+{
+  StateRecordHeader h;
+  std::memcpy(&h, rec, sizeof h);
+  const StateRecordHeader& want = m->record_header;
+  const std::string at = "record " + std::to_string(i) + " (stream " + std::to_string(stream) + "): ";
+  char hex[2][24];
+  std::snprintf(hex[0], sizeof hex[0], "%016llx", (unsigned long long)h.fingerprint);
+  std::snprintf(hex[1], sizeof hex[1], "%016llx", (unsigned long long)want.fingerprint);
+  if (std::memcmp(h.magic, "NAMS", 4) != 0)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "magic is not \"NAMS\": not a stream state record");
+  if (h.version != kStateRecordVersion)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "format version " + std::to_string(h.version) + " (this library reads "
+                                                 + std::to_string(kStateRecordVersion) + ")");
+  if (h.architecture != want.architecture)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "architecture " + std::to_string(h.architecture) + ", the model's is "
+                                                 + std::to_string(want.architecture));
+  if (h.payload_floats != want.payload_floats)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "payload float count " + std::to_string(h.payload_floats)
+                                                 + ", the model's record holds " + std::to_string(want.payload_floats));
+  if (h.fingerprint != want.fingerprint)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "model fingerprint " + hex[0] + " is not this model's (" + hex[1]
+                                                 + "): a record of another model, or of another slimmable size");
+  return NAM_B200_OK;
+}
+
+// host records go through device staging in groups of at most this many bytes
+constexpr size_t kRecordStagingBytes = (size_t)64 << 20;
 
 } // namespace
 
@@ -2367,6 +2672,13 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
     if (m->opts.prewarm_on_reset)
       prewarm(m);
     CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
+    // every stream is now in the state of a freshly reset one: keep stream 0's record for nam_b200_reset_streams (an LSTM
+    // keeps its running state across a Reset, so its streams are re-derived per call instead)
+    if (m->spec.arch != Arch::LSTM && m->state_error.empty())
+    {
+      const int32_t s0 = 0;
+      export_records(m, &s0, 1, m->d_fresh, 0, m->stream);
+    }
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
     m->timing_valid = true;
     return NAM_B200_OK;
@@ -2382,6 +2694,210 @@ int nam_b200_prewarm(nam_b200_model* m)
     prewarm(m);
     return NAM_B200_OK;
   });
+}
+
+// ---- per-stream state control ---------------------------------------------------------------------------------------
+int64_t nam_b200_stream_state_size(const nam_b200_model* m)
+{
+  m = active_model(m);
+  if (!m)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null model handle");
+  if (!m->state_error.empty())
+    return fail(NAM_B200_ERR_UNSUPPORTED, "no per-stream state records for this handle: " + m->state_error);
+  return (int64_t)record_bytes(m);
+}
+
+int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int fresh)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "reset_streams");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "streams", true);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    if (m->spec.arch == Arch::LSTM)
+      lstm_reset_rows(m, streams, n, fresh != 0);
+    else
+      import_records(m, streams, n, m->d_fresh, 0, m->stream); // (fresh or not: Reset forgets the past)
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_copy_streams(nam_b200_model* m, const int32_t* src, const int32_t* dst, int n)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "copy_streams");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, src, n, "src", false);
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, dst, n, "dst", true);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    // gather every source row into scratch, then scatter: overlapping lists (a swap) see the sources as they were
+    const size_t rows = (size_t)n * (size_t)m->state_stride;
+    const bool linear = m->spec.arch == Arch::Linear && m->d_state_tmp;
+    ensure_xfer(m, rows * sizeof(float) * (linear ? 2 : 1));
+    std::vector<StreamRef> refs((size_t)2 * n);
+    for (int i = 0; i < n; i++)
+    {
+      refs[(size_t)i] = StreamRef{src[i], 0, 0, 0};
+      refs[(size_t)(n + i)] = StreamRef{dst[i], 0, 0, 0};
+    }
+    const StreamRef* d_refs = upload_refs(m, refs, m->stream);
+    float* scratch = reinterpret_cast<float*>(m->d_xfer);
+    copy_rows(m, scratch, nullptr, m->d_state, d_refs, n, m->stream);
+    copy_rows(m, m->d_state, d_refs + n, scratch, nullptr, n, m->stream);
+    if (linear) // both buffers of the double buffer; the destination keeps the source's buffer parity
+    {
+      copy_rows(m, scratch + rows, nullptr, m->d_state_tmp, d_refs, n, m->stream);
+      copy_rows(m, m->d_state_tmp, d_refs + n, scratch + rows, nullptr, n, m->stream);
+    }
+    std::vector<uint32_t> clock((size_t)n), flips((size_t)n);
+    for (int i = 0; i < n; i++)
+    {
+      clock[(size_t)i] = m->stream_clock[(size_t)src[i]];
+      flips[(size_t)i] = m->stream_flips[(size_t)src[i]];
+    }
+    for (int i = 0; i < n; i++)
+    {
+      m->stream_clock[(size_t)dst[i]] = clock[(size_t)i];
+      m->stream_flips[(size_t)dst[i]] = flips[(size_t)i];
+    }
+    m->streams_identical = false;
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_export_streams(nam_b200_model* m, const int32_t* streams, int n, void* dst, int64_t record_stride)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "export_streams");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "streams", false);
+    if (rc == NAM_B200_OK)
+      rc = check_records(m, dst, n, record_stride, false);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    const size_t rb = record_bytes(m);
+    const int group = (int)std::max<size_t>(1, kRecordStagingBytes / rb);
+    ensure_xfer(m, (size_t)std::min(n, group) * rb);
+    for (int i0 = 0; i0 < n; i0 += group)
+    {
+      const int k = std::min(group, n - i0);
+      export_records(m, streams + i0, k, m->d_xfer, (long)rb, m->stream);
+      CUDA_CHECK(cudaMemcpy2DAsync(static_cast<unsigned char*>(dst) + (size_t)i0 * record_stride, (size_t)record_stride, m->d_xfer,
+                                   rb, rb, (size_t)k, cudaMemcpyDeviceToHost, m->stream));
+      CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    }
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_import_streams(nam_b200_model* m, const int32_t* streams, int n, const void* src, int64_t record_stride)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "import_streams");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "streams", true);
+    if (rc == NAM_B200_OK)
+      rc = check_records(m, src, n, record_stride, false);
+    for (int i = 0; i < n && rc == NAM_B200_OK; i++)
+      rc = check_record_header(m, static_cast<const unsigned char*>(src) + (size_t)i * record_stride, i, streams[i]);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    const size_t rb = record_bytes(m);
+    const int group = (int)std::max<size_t>(1, kRecordStagingBytes / rb);
+    ensure_xfer(m, (size_t)std::min(n, group) * rb);
+    for (int i0 = 0; i0 < n; i0 += group)
+    {
+      const int k = std::min(group, n - i0);
+      CUDA_CHECK(cudaMemcpy2DAsync(m->d_xfer, rb, static_cast<const unsigned char*>(src) + (size_t)i0 * record_stride,
+                                   (size_t)record_stride, rb, (size_t)k, cudaMemcpyHostToDevice, m->stream));
+      import_records(m, streams + i0, k, m->d_xfer, (long)rb, m->stream);
+      CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    }
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_export_streams_device(nam_b200_model* m, const int32_t* streams, int n, void* dst_device, int64_t record_stride,
+                                   void* cuda_stream)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "export_streams_device");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "streams", false);
+    if (rc == NAM_B200_OK)
+      rc = check_records(m, dst_device, n, record_stride, true);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    const cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
+    export_records(m, streams, n, static_cast<unsigned char*>(dst_device), (long)record_stride, st);
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, int n, const void* src_device,
+                                   int64_t record_stride, void* cuda_stream)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "import_streams_device");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "streams", true);
+    if (rc == NAM_B200_OK)
+      rc = check_records(m, src_device, n, record_stride, true);
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    const cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
+    // the headers come to the host and are checked before anything is launched
+    std::vector<unsigned char> headers((size_t)n * kStateHeaderBytes);
+    CUDA_CHECK(cudaMemcpy2DAsync(headers.data(), kStateHeaderBytes, src_device, (size_t)record_stride, kStateHeaderBytes, (size_t)n,
+                                 cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; i++)
+    {
+      rc = check_record_header(m, headers.data() + (size_t)i * kStateHeaderBytes, i, streams[i]);
+      if (rc != NAM_B200_OK)
+        return rc;
+    }
+    import_records(m, streams, n, static_cast<const unsigned char*>(src_device), (long)record_stride, st);
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t capacity)
+{
+  if (!nam_json_text || !out || capacity <= 0)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument or empty output buffer");
+  try
+  {
+    LoadOptions lo;
+    ModelSpec ms = model_spec_from_text(nam_json_text, lo);
+    if (ms.arch == Arch::Container) // the default (largest) sub-model, the one a new handle serves
+      ms = model_spec_from_text(ms.submodels.back().model_json, lo);
+    const std::string s = state_layout_json(ms);
+    if ((int64_t)s.size() >= capacity)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "the state layout needs " + std::to_string(s.size() + 1) + " bytes, the buffer has "
+                                                   + std::to_string(capacity));
+    std::memcpy(out, s.c_str(), s.size() + 1);
+    return NAM_B200_OK;
+  }
+  catch (const json::ParseError& ex)
+  {
+    return fail(NAM_B200_ERR_FILE, ex.what());
+  }
+  catch (const std::exception& ex)
+  {
+    return fail(NAM_B200_ERR_MODEL, ex.what());
+  }
 }
 
 int nam_b200_process_f32_device(nam_b200_model* m, const float* in_device, float* out_device, int batch, int n_frames,
@@ -2452,6 +2968,7 @@ int nam_b200_process_f32(nam_b200_model* m, const float* in, float* out, int bat
                                      (size_t)nb, cudaMemcpyDeviceToHost, m->copy_out));
       }
       m->t_base += (uint32_t)n_frames;
+      std::fill(m->stream_clock.begin(), m->stream_clock.begin() + batch, m->t_base);
       m->streams_identical = false;
       CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
       CUDA_CHECK(cudaStreamSynchronize(m->copy_out));

@@ -965,6 +965,70 @@ void build_slimmable_wavenet(ModelSpec& ms, const json::Value& root, const json:
   }
 }
 
+// ---- model fingerprint (ModelSpec::fingerprint) ----------------------------------------------
+struct Fnv64
+{
+  uint64_t h = 0xcbf29ce484222325ull;
+  void bytes(const void* p, size_t n)
+  {
+    const unsigned char* c = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < n; i++)
+      h = (h ^ c[i]) * 0x100000001b3ull;
+  }
+  void u64(uint64_t v) { bytes(&v, sizeof v); }
+  void str(const std::string& s)
+  {
+    u64(s.size());
+    bytes(s.data(), s.size());
+  }
+  // canonical walk: a type tag per value, object members in key order
+  void value(const json::Value& v)
+  {
+    u64((uint64_t)v.type());
+    switch (v.type())
+    {
+      case json::Value::Type::Null: break;
+      case json::Value::Type::Bool: u64(v.as_bool() ? 1 : 0); break;
+      case json::Value::Type::Number:
+      {
+        const double d = v.as_double();
+        bytes(&d, sizeof d);
+        break;
+      }
+      case json::Value::Type::String: str(v.as_string()); break;
+      case json::Value::Type::Array:
+        u64(v.size());
+        for (const auto& item : v.items())
+          value(item);
+        break;
+      case json::Value::Type::Object:
+      {
+        std::vector<const std::pair<std::string, json::Value>*> members;
+        for (const auto& kv : v.members())
+          members.push_back(&kv);
+        std::sort(members.begin(), members.end(), [](auto* a, auto* b) { return a->first < b->first; });
+        u64(members.size());
+        for (auto* kv : members)
+        {
+          str(kv->first);
+          value(kv->second);
+        }
+        break;
+      }
+    }
+  }
+};
+
+uint64_t model_fingerprint(const std::string& architecture, const json::Value& config, const std::vector<float>& weights)
+{
+  Fnv64 f;
+  f.str(architecture);
+  f.value(config);
+  f.u64(weights.size());
+  f.bytes(weights.data(), weights.size() * sizeof(float));
+  return f.h;
+}
+
 ModelSpec build_spec(const json::Value& root, const LoadOptions& opts)
 {
   if (!root.is_object())
@@ -1004,6 +1068,7 @@ ModelSpec build_spec(const json::Value& root, const LoadOptions& opts)
     ms.output_level = extract("output_level_dbu");
   }
   const json::Value& config = root.at("config");
+  ms.fingerprint = model_fingerprint(ms.architecture, config, weights);
   if (ms.architecture == "WaveNet" && config_is_slimmable_wavenet(config))
     build_slimmable_wavenet(ms, root, config, weights, opts);
   else if (ms.architecture == "WaveNet")

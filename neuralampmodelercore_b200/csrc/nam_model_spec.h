@@ -12,6 +12,7 @@
 // No CUDA here: everything in this file runs once at load time on the host.
 #pragma once
 
+#include <cstdint>
 #include <memory>
 #include <optional>
 #include <stdexcept>
@@ -209,6 +210,10 @@ struct ModelSpec
   int prewarm_samples = 0; // DSP::GetPrewarmSamples()
   std::optional<double> loudness, input_level, output_level;
   size_t n_weights = 0;
+  // FNV-1a 64 over the architecture name, the parsed "config" object (keys sorted, numbers as double bits) and the
+  // float32 bits of the weights: the identity of a model's state layout and arithmetic, independent of load options
+  // (fast_tanh) and of how the document was spelled.  Stamped into per-stream state records (stream_state.h).
+  uint64_t fingerprint = 0;
   WaveNetSpec wavenet;
   LstmSpec lstm;
   LinearSpec linear;

@@ -317,6 +317,73 @@ class DSP:
         if rc != 0:
             _raise(rc, self._lib)
 
+    # ---- per-stream state (include/nam_b200.h: records, per-stream clocks) ------------------------------------------
+    @property
+    def state_record_bytes(self) -> int:
+        """Bytes of one stream's state record (64-byte header + float32 payload)."""
+        n = int(self._lib.nam_b200_stream_state_size(self._h))
+        if n < 0:
+            _raise(n, self._lib)
+        return n
+
+    @staticmethod
+    def _streams(streams) -> np.ndarray:
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(streams)), dtype=np.int32)
+
+    @staticmethod
+    def _i32p(a: np.ndarray):
+        return a.ctypes.data_as(C.POINTER(C.c_int32))
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            _raise(rc, self._lib)
+
+    def reset_streams(self, streams, fresh: bool = False) -> None:
+        """DSP::Reset for the listed streams only (the others are untouched).  LSTM: fresh=False keeps h, c and prewarms
+        on top of them (what Reset does); fresh=True starts from the trained initial state like a new handle."""
+        s = self._streams(streams)
+        self._check(self._lib.nam_b200_reset_streams(self._h, self._i32p(s), len(s), int(bool(fresh))))
+
+    def copy_streams(self, src, dst) -> None:
+        """dst[i] takes src[i]'s state; the sources are all read first, so a swap works."""
+        s, d = self._streams(src), self._streams(dst)
+        if len(s) != len(d):
+            raise ValueError("src and dst must list the same number of streams")
+        self._check(self._lib.nam_b200_copy_streams(self._h, self._i32p(s), self._i32p(d), len(s)))
+
+    def export_streams(self, streams) -> np.ndarray:
+        """The listed streams' state records -> uint8 array (n, state_record_bytes)."""
+        s = self._streams(streams)
+        rb = self.state_record_bytes
+        out = np.zeros((len(s), rb), np.uint8)
+        self._check(self._lib.nam_b200_export_streams(self._h, self._i32p(s), len(s), out.ctypes.data_as(C.c_void_p), rb))
+        return out
+
+    def import_streams(self, streams, records: np.ndarray) -> None:
+        """Records (one row each, as export_streams returns them) -> the listed streams."""
+        s = self._streams(streams)
+        r = np.asarray(records)
+        if r.ndim == 1:
+            r = r[None, :]
+        if r.dtype != np.uint8 or r.ndim != 2 or r.shape[0] != len(s):
+            raise ValueError("records must be a uint8 array with one row per stream")
+        r = np.ascontiguousarray(r)
+        self._check(self._lib.nam_b200_import_streams(self._h, self._i32p(s), len(s), r.ctypes.data_as(C.c_void_p), r.shape[1]))
+
+    def export_streams_device(self, streams, dst_ptr: int, record_stride: int | None = None, cuda_stream: int = 0) -> None:
+        """Records into device memory at dst_ptr (e.g. torch.Tensor.data_ptr()), asynchronous on `cuda_stream`."""
+        s = self._streams(streams)
+        stride = int(record_stride if record_stride is not None else self.state_record_bytes)
+        self._check(self._lib.nam_b200_export_streams_device(self._h, self._i32p(s), len(s), C.c_void_p(dst_ptr), stride,
+                                                             C.c_void_p(cuda_stream) if cuda_stream else None))
+
+    def import_streams_device(self, streams, src_ptr: int, record_stride: int | None = None, cuda_stream: int = 0) -> None:
+        """Records from device memory -> the listed streams; the headers are checked on the host before any launch."""
+        s = self._streams(streams)
+        stride = int(record_stride if record_stride is not None else self.state_record_bytes)
+        self._check(self._lib.nam_b200_import_streams_device(self._h, self._i32p(s), len(s), C.c_void_p(src_ptr), stride,
+                                                             C.c_void_p(cuda_stream) if cuda_stream else None))
+
 
 def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: Optional[bool], ctas_per_sm: int,
              kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0):
@@ -390,6 +457,21 @@ def inspect(config, fast_tanh: Optional[bool] = None) -> dict:
     else:
         text = config if isinstance(config, str) else json.dumps(config)
         rc = lib.nam_b200_inspect_json(text.encode(), ft, buf, len(buf))
+    if rc != 0:
+        _raise(rc, lib)
+    return json.loads(buf.value.decode())
+
+
+def state_layout(config) -> dict:
+    """Host-only: the per-stream state record of a .nam (path, dict or JSON text): architecture, header_bytes,
+    payload_floats, record_bytes, fingerprint and segments [{name, channels, columns, offset}].  Needs no GPU."""
+    import json
+
+    lib = _capi.load()
+    text = (Path(config).read_text() if isinstance(config, os.PathLike) or (isinstance(config, str) and not config.lstrip().startswith("{"))
+            else (config if isinstance(config, str) else json.dumps(config))).encode()
+    buf = C.create_string_buffer(1 << 20)
+    rc = lib.nam_b200_state_layout_json(text, buf, len(buf))
     if rc != 0:
         _raise(rc, lib)
     return json.loads(buf.value.decode())
