@@ -132,9 +132,10 @@ int nam_b200_prewarm(nam_b200_model* m);
  * record carries: a record taken at one slimmable size is refused at another.
  *
  * The handle keeps, per stream, the clock value at which the stream's history ends.  A stream left out of process calls
- * (batch < max_batch) keeps its history at that older point: export reads it there, correctly; but process_* reads every
- * stream at the handle's current clock, so such a stream must be brought back with export + import, or with
- * nam_b200_reset_streams, before it takes part in a call again.
+ * (batch < max_batch, or not listed in nam_b200_process_streams_f32) keeps its history at that older point: export reads it
+ * there, and every process call that includes it again continues from its own clock -- a pause needs no export, import or
+ * reset.  (Contiguous calls launch exactly as before while every stream in [0, batch) is in step with the handle; otherwise
+ * they carry the per-stream clocks like nam_b200_process_streams_f32.)
  *
  * Stream lists hold indices in [0, max_batch); destinations must be distinct.  Everything is checked on the host before
  * anything runs (NAM_B200_ERR_INVALID_ARGUMENT with the offending stream and field; NAM_B200_ERR_STATE before reset). */
@@ -177,6 +178,20 @@ int nam_b200_process_f32(nam_b200_model* m, const float* in, float* out, int bat
  * No copies, no synchronisation. */
 int nam_b200_process_f32_device(nam_b200_model* m, const float* in_device, float* out_device, int batch, int n_frames,
                                 int64_t in_stride, int64_t out_stride, void* cuda_stream);
+
+/* Streams streams[0..n) (distinct, in [0, max_batch), any order): row i of in / out belongs to streams[i]
+ * (in + i*in_stride, channel planes back to back as in nam_b200_process_f32).  Each listed stream continues from its
+ * own history, wherever its clock stands; unlisted streams are untouched.  Host pointers; returns when `out` is filled.
+ * The kernel is the one a contiguous call of batch = n would get.  Afterwards each listed stream's clock, and the
+ * handle's, has moved on by n_frames.  Everything is checked on the host before anything is queued (NAM_B200_ERR_STATE
+ * before reset; NAM_B200_ERR_INVALID_ARGUMENT naming the stream or field); n == 0 or n_frames == 0 does nothing. */
+int nam_b200_process_streams_f32(nam_b200_model* m, const int32_t* streams, int n, const float* in, float* out,
+                                 int n_frames, int64_t in_stride, int64_t out_stride);
+/* The same on device audio buffers, asynchronous on cuda_stream (NULL = the handle's stream).  `streams` is a host
+ * array and may be reused as soon as the call returns. */
+int nam_b200_process_streams_f32_device(nam_b200_model* m, const int32_t* streams, int n, const float* in_device,
+                                        float* out_device, int n_frames, int64_t in_stride, int64_t out_stride,
+                                        void* cuda_stream);
 
 /* Host-buffer contract of nam_b200_process_f32: any host memory is accepted; with PAGE-LOCKED buffers (cudaMallocHost,
  * cudaHostRegister, or nam_b200_pin_host_buffer below) the call pipelines host->device copy, kernel and device->host copy

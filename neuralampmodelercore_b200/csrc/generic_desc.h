@@ -18,6 +18,17 @@ typedef unsigned int uint32_t;
 namespace namb200
 {
 
+// One stream of a launch that addresses streams through a table: the state row it uses and the clock at which that row's
+// history ends.  The process kernels' slot tables (position i of the call -> slots[i]) and the pack / unpack launches of
+// stream_state.cuh share it; the NVRTC-compiled kernels declare a layout twin (SlotRef).
+struct StreamRef
+{
+  int stream;
+  uint32_t clock; // the handle clock at which the stream's history ends (pack, process) or will end (unpack)
+  int alt; // Linear: the stream's history is in the alternate buffer of the double buffer
+  int pad;
+};
+
 constexpr int kGenMaxVec = 64; // widest per-frame vector (channels, 2 x bottleneck, condition, head sizes)
 constexpr int kGenMaxArrays = 4;
 constexpr int kGenMaxHeadConvs = 8;
@@ -103,6 +114,7 @@ struct ConvNetKernelParams
   int batch, n_frames;
   uint32_t t_base;
   int n_weight_floats;
+  const StreamRef* slots; // nullptr: position i is state row i at t_base; else row slots[i].stream at slots[i].clock
 };
 
 struct GenericKernelParams
@@ -120,6 +132,7 @@ struct GenericKernelParams
   int batch, n_frames;
   uint32_t t_base;
   int n_weight_floats; // multiple of 4; the kernel keeps the blob in shared memory when it was given the room
+  const StreamRef* slots; // as ConvNetKernelParams::slots
 };
 
 } // namespace namb200

@@ -58,6 +58,7 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
 
   const int stream = blockIdx.x * SPC + sl;
   const bool live = stream < p.batch;
+  const size_t row = p.slots ? (size_t)p.slots[live ? stream : 0].stream : (size_t)stream; // state row of this position
   // this lane's units (clamped: surplus lanes shadow the last unit and are never read)
   int unit[UPL];
   bool owns[UPL];
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
       c[l][k] = 0.0f;
       if (l < L && live)
       {
-        const float* st = p.state + (size_t)stream * p.state_stride + (size_t)l * 2 * H;
+        const float* st = p.state + row * p.state_stride + (size_t)l * 2 * H;
         h[l][k] = st[unit[k]];
         c[l][k] = st[H + unit[k]];
       }
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
       for (int k = 0; k < UPL; k++)
         if (l < L && owns[k])
         {
-          float* st = p.state + (size_t)stream * p.state_stride + (size_t)l * 2 * H;
+          float* st = p.state + row * p.state_stride + (size_t)l * 2 * H;
           st[unit[k]] = h[l][k];
           st[H + unit[k]] = c[l][k];
         }

@@ -24,6 +24,14 @@
 namespace namb200_lstm_spec
 {
 
+// layout twin of namb200::StreamRef (generic_desc.h): one entry of a call's slot table (an LSTM has no clock)
+struct SlotRef
+{
+  int stream;
+  unsigned clock;
+  int alt, pad;
+};
+
 struct LstmSpecParams
 {
   float* state; // [batch][state_stride]
@@ -32,6 +40,9 @@ struct LstmSpecParams
   float* out;
   long in_stride, out_stride;
   int batch, n_frames;
+  // slot table (nullptr: position b is state row b): position b uses row slots[b].stream; inputs and outputs stay
+  // indexed by position
+  const SlotRef* slots;
 };
 
 __device__ __forceinline__ float rcp_approx(float x)
@@ -88,6 +99,7 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
   const int stream0 = blockIdx.x * kTile;
   const int stream = stream0 + lane;
   const bool live = stream < p.batch;
+  const int row = p.slots ? p.slots[min(stream, p.batch - 1)].stream : min(stream, p.batch - 1); // state row
 
   float h[L][H], c[L][H];
 #pragma unroll
@@ -95,7 +107,7 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
 #pragma unroll
     for (int u = 0; u < H; u++)
     {
-      const float* st = p.state + (size_t)min(stream, p.batch - 1) * p.state_stride + l * 2 * H;
+      const float* st = p.state + (size_t)row * p.state_stride + l * 2 * H;
       h[l][u] = st[u];
       c[l][u] = st[H + u];
     }
@@ -202,7 +214,7 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
 #pragma unroll
       for (int u = 0; u < H; u++)
       {
-        float* st = p.state + (size_t)stream * p.state_stride + l * 2 * H;
+        float* st = p.state + (size_t)row * p.state_stride + l * 2 * H;
         st[u] = h[l][u];
         st[H + u] = c[l][u];
       }
@@ -228,6 +240,7 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
   const int stream0 = blockIdx.x * SPW;
   const int stream = stream0 + grp;
   const bool live = stream < p.batch;
+  const int row = p.slots ? p.slots[min(stream, p.batch - 1)].stream : min(stream, p.batch - 1); // state row
   const unsigned base_lane = (unsigned)(lane & ~3);
 
   // my gate's rows: W[q*H + u][0 .. I+H) and b[q*H + u].  Fast regime: the 0.5 z of the sigmoid gates is folded in.
@@ -269,7 +282,7 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
 #pragma unroll
     for (int u = 0; u < H; u++)
     {
-      const float* st = p.state + (size_t)min(stream, p.batch - 1) * p.state_stride + l * 2 * H;
+      const float* st = p.state + (size_t)row * p.state_stride + l * 2 * H;
       h[l][u] = st[u];
       c[l][u] = st[H + u];
     }
@@ -350,7 +363,7 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
 #pragma unroll
       for (int u = 0; u < H; u++)
       {
-        float* st = p.state + (size_t)stream * p.state_stride + l * 2 * H;
+        float* st = p.state + (size_t)row * p.state_stride + l * 2 * H;
         st[u] = h[l][u];
         st[H + u] = c[l][u];
       }

@@ -93,6 +93,8 @@ struct LstmKernelParams
   // multi-channel models (lstm.cpp:103-125): stream b's channel c is the plane in[b * in_stride + c * n_frames ..];
   // input_size == in_channels.  Mono models take the staged (coalesced) path, in_ch == out_ch == 1.
   int in_ch, out_ch;
+  // slot table (nullptr: position b is state row b): position b uses state row slots[b].stream; in / out stay by position
+  const StreamRef* slots;
 };
 
 constexpr int kLstmThreads = 64; // streams per CTA
@@ -123,10 +125,11 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
     sw[i] = __ldg(p.weights + i);
   const int stream = blockIdx.x * kLstmThreads + tid;
   const bool active = stream < p.batch;
+  const size_t row = p.slots ? (size_t)p.slots[active ? stream : 0].stream : (size_t)stream;
   const int n_state = p.num_layers * 2 * H;
   if (active)
     for (int i = 0; i < n_state; i++)
-      sstate[i * kLstmThreads + tid] = p.state[(size_t)stream * p.state_stride + i];
+      sstate[i * kLstmThreads + tid] = p.state[row * p.state_stride + i];
   __syncthreads();
 
   const int stream0 = blockIdx.x * kLstmThreads;
@@ -221,7 +224,7 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
   }
   if (active)
     for (int i = 0; i < n_state; i++)
-      p.state[(size_t)stream * p.state_stride + i] = sstate[i * kLstmThreads + tid];
+      p.state[row * p.state_stride + i] = sstate[i * kLstmThreads + tid];
 }
 
 } // namespace
@@ -245,6 +248,10 @@ struct LinearKernelParams
   float* __restrict__ out;
   long in_stride, out_stride;
   int batch, n_frames;
+  // slot table (nullptr: position b is row b of `state`): position b uses row slots[b].stream of `state`, or of `state_alt`
+  // when slots[b].alt -- each stream reads the buffer it was last written to and the update writes the other one
+  const StreamRef* slots;
+  float* __restrict__ state_alt;
 };
 
 constexpr int kLinThreads = 256;
@@ -261,7 +268,8 @@ __global__ void __launch_bounds__(kLinThreads) linear_kernel(const LinearKernelP
   for (int i = tid; i < p.rf; i += kLinThreads)
     sw[i] = __ldg(p.impulse + i);
   const float* xin = p.in + (size_t)stream * p.in_stride;
-  const float* st = p.state + (size_t)stream * p.state_stride;
+  const float* st = p.slots ? (p.slots[stream].alt ? p.state_alt : p.state) + (size_t)p.slots[stream].stream * p.state_stride
+                            : p.state + (size_t)stream * p.state_stride;
   for (int i = tid; i < hist + kLinThreads; i += kLinThreads)
   {
     const int t = t0 - hist + i; // frame index relative to this call
@@ -284,7 +292,7 @@ __global__ void __launch_bounds__(kLinThreads) linear_kernel(const LinearKernelP
   }
 }
 
-// new_state = last (rf-1) samples of [old_state | in[0:n)]
+// new_state = last (rf-1) samples of [old_state | in[0:n)] (slot table: into the other buffer of each stream's pair)
 __global__ void linear_update_state_kernel(const LinearKernelParams p, float* __restrict__ new_state)
 {
   const int hist = p.rf - 1;
@@ -293,12 +301,20 @@ __global__ void linear_update_state_kernel(const LinearKernelParams p, float* __
   if (i >= hist)
     return;
   const int t = p.n_frames - hist + i; // relative frame index of new history slot i
+  const float* old_st = p.state + (size_t)stream * p.state_stride;
+  float* new_st = new_state + (size_t)stream * p.state_stride;
+  if (p.slots)
+  {
+    const StreamRef r = p.slots[stream];
+    old_st = (r.alt ? p.state_alt : p.state) + (size_t)r.stream * p.state_stride;
+    new_st = (r.alt ? p.state : p.state_alt) + (size_t)r.stream * p.state_stride;
+  }
   float v;
   if (t >= 0)
     v = p.in[(size_t)stream * p.in_stride + t];
   else
-    v = p.state[(size_t)stream * p.state_stride + hist + t];
-  new_state[(size_t)stream * p.state_stride + i] = v;
+    v = old_st[hist + t];
+  new_st[i] = v;
 }
 
 // =================================================================================================
@@ -433,6 +449,14 @@ struct nam_b200_model
   std::string state_error; // non-empty: the stream-state calls are refused with this reason
   unsigned char* d_fresh = nullptr; // WaveNet / ConvNet / Linear: the record of a stream straight after nam_b200_reset
   StreamRef* d_refs = nullptr; // stream lists of pack / unpack / row-copy launches
+  // slot tables of process calls (nam_b200_process_streams_f32, and contiguous calls over a stream that sat out calls):
+  // position i of the call -> state row, clock and Linear buffer.  The host copy is rebuilt per call; the device copy
+  // (max_batch entries) is rewritten only once the previous table call's kernels, on whichever CUDA stream, are done with it
+  std::vector<StreamRef> h_slots;
+  StreamRef* d_slots = nullptr;
+  cudaEvent_t slots_free = nullptr; // recorded after the last launch that reads d_slots
+  bool slots_used = false;
+  int n_out_of_phase = 0; // streams whose history does not end at t_base (Linear: or sits in the other buffer)
   size_t refs_capacity = 0;
   unsigned char* d_xfer = nullptr; // staging of host records, scratch rows of copies and LSTM prewarms
   size_t xfer_bytes = 0;
@@ -484,6 +508,10 @@ struct nam_b200_model
       cudaFree(d_fresh);
     if (d_refs)
       cudaFree(d_refs);
+    if (d_slots)
+      cudaFree(d_slots);
+    if (slots_free)
+      cudaEventDestroy(slots_free);
     if (d_xfer)
       cudaFree(d_xfer);
     if (d_in)
@@ -532,10 +560,12 @@ constexpr WnGeometry kWnGeom[4] = {{128, 3, 8}, {256, 2, 9}, {128, 3, 6}, {256, 
 // calls of up to this many frames take the multi-stream geometry 2 / 3
 constexpr int kWnShortMaxFrames[2] = {96, 192};
 
+// (calls with a slot table run the kernel's TBL instantiation; the occupancy queries take the lower of the two, so that the
+// co-residency the tile-parallel modes rely on holds for both)
 template <int C0, int C1, int NT, int MINB, int LQ>
 void launch_wavenet_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
 {
-  auto kern = wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>;
+  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ, false, true> : wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>;
   ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
   kern<<<grid, NT, smem, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
@@ -544,12 +574,16 @@ void launch_wavenet_variant(nam_b200_model* m, const WaveNetKernelParams& kp, in
 template <int C0, int C1, int NT, int MINB, int LQ>
 int occupancy_wavenet_variant(size_t smem)
 {
-  auto kern = wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NT, smem) != cudaSuccess)
-    return 1;
-  return n > 0 ? n : 1;
+  int best = 1 << 30;
+  for (auto kern : {wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>, wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ, false, true>})
+  {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NT, smem) != cudaSuccess)
+      return 1;
+    best = std::min(best, n);
+  }
+  return best > 0 ? best : 1;
 }
 
 // lock-step tile-parallel kernels (LS = true), one stream per tile.
@@ -570,7 +604,7 @@ constexpr LsGeometry kLsGeom[kLsGeoms] = {{128, 2, 3, 8}, {256, 2, 2, 9}, {128, 
 template <int C0, int C1, int S, int NT, int MINB, int LQ>
 void launch_wavenet_ls_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
 {
-  auto kern = wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>;
+  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true, true> : wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>;
   ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
   // The tiles spin on each other's flags, so they must all be resident at once: a cooperative launch is
   // gang-scheduled (it starts only when the whole grid fits), which keeps two such launches from different handles
@@ -582,12 +616,16 @@ void launch_wavenet_ls_variant(nam_b200_model* m, const WaveNetKernelParams& kp,
 template <int C0, int C1, int S, int NT, int MINB, int LQ>
 int occupancy_wavenet_ls_variant(size_t smem)
 {
-  auto kern = wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NT, smem) != cudaSuccess)
-    return 1;
-  return n > 0 ? n : 1;
+  int best = 1 << 30;
+  for (auto kern : {wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>, wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true, true>})
+  {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NT, smem) != cudaSuccess)
+      return 1;
+    best = std::min(best, n);
+  }
+  return best > 0 ? best : 1;
 }
 
 #define WN_LS_CASE(C0, C1, FN, ...)                                                                                  \
@@ -690,13 +728,13 @@ void launch_wavenet_lat2_variant(nam_b200_model* m, const WaveNetKernelParams& k
 {
   if (fw == 2)
   {
-    auto kern = wavenet_lat2_kernel<C0, C1, 2>;
+    auto kern = kp.slots ? wavenet_lat2_kernel<C0, C1, 2, true> : wavenet_lat2_kernel<C0, C1, 2>;
     ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024); // (+ 520 B of static mbarriers)
     kern<<<kp.batch, 256, smem, st>>>(kp);
   }
   else
   {
-    auto kern = wavenet_lat2_kernel<C0, C1, 4>;
+    auto kern = kp.slots ? wavenet_lat2_kernel<C0, C1, 4, true> : wavenet_lat2_kernel<C0, C1, 4>;
     ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
     kern<<<kp.batch, 512, smem, st>>>(kp);
   }
@@ -719,7 +757,8 @@ constexpr int kSmallNt = 128, kSmallLq = 7;
 template <int C0, int C1>
 void launch_wavenet_small_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
 {
-  auto kern = wavenet_fused_kernel<C0, C1, 1, kSmallNt, 3, kSmallLq, false>;
+  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, 1, kSmallNt, 3, kSmallLq, false, true>
+                       : wavenet_fused_kernel<C0, C1, 1, kSmallNt, 3, kSmallLq, false>;
   ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
   kern<<<grid, kSmallNt, smem, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
@@ -871,6 +910,7 @@ struct SpecKernelParams
   uint32_t t_base;
   float* scratch; // stream-pair variant (S = 2) only: per-CTA interleaved rings; the shipped geometry is S = 1
   long scratch_stride;
+  const StreamRef* slots; // slot table (namb200_spec::SlotRef), nullptr = rows [0, batch) at t_base; never with S = 2
 };
 
 int jit_mode(const nam_b200_model* m);
@@ -884,6 +924,7 @@ struct GenSpecKernelParams // mirror of namb200_gspec::GParams
   long in_stride, out_stride;
   int batch, n_frames;
   unsigned t_base;
+  const StreamRef* slots;
 };
 
 
@@ -1023,6 +1064,7 @@ struct LatKernelParams // mirror of namb200_lat::LatParams
   uint32_t t_base;
   unsigned* done_flag;
   unsigned seq;
+  const StreamRef* slots;
 };
 
 // reset(): plugin-style handles (few streams, maxBufferSize <= 128) get the low-latency kernel for calls of up to
@@ -1086,7 +1128,7 @@ void launch_wavenet_lat(nam_b200_model* m, const WaveNetKernelParams& kp, cudaSt
   if (flag)
     m->flag_seq++;
   LatKernelParams lp{kp.state, kp.state_stride, kp.in, kp.out, kp.in_stride, kp.out_stride, kp.batch, kp.n_frames, kp.t_base,
-                     flag, m->flag_seq};
+                     flag, m->flag_seq, kp.slots};
   m->flag_pending = flag != nullptr;
   void* args[] = {&lp};
   CUDA_CHECK(cudaLaunchKernel((const void*)m->lat_kernel, dim3(kp.batch), dim3(m->lat_threads), args, m->lat_smem, st));
@@ -1095,7 +1137,7 @@ void launch_wavenet_lat(nam_b200_model* m, const WaveNetKernelParams& kp, cudaSt
 void launch_wavenet_spec(nam_b200_model* m, const WaveNetKernelParams& kp, cudaStream_t st)
 {
   SpecKernelParams sp{kp.state, kp.state_stride, kp.in,  kp.out, kp.in_stride, kp.out_stride,
-                      kp.batch, kp.n_frames,     kp.t_base, nullptr, 0};
+                      kp.batch, kp.n_frames,     kp.t_base, nullptr, 0, kp.slots};
   void* args[] = {&sp};
   int grid = std::min(kp.batch, m->spec_ctas_per_sm * std::max(1, m->sm_count - m->reserved_sms));
   if (grid < 1)
@@ -1103,13 +1145,14 @@ void launch_wavenet_spec(nam_b200_model* m, const WaveNetKernelParams& kp, cudaS
   CUDA_CHECK(cudaLaunchKernel((const void*)m->spec_kernel, dim3(grid), dim3(m->spec_geom.nt), args, m->spec_smem, st));
 }
 
+// `slots`: the call's slot table (position b -> state row, clock), nullptr = rows stream0 + b at t_base
 void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                    long out_stride, cudaStream_t st, int stream0 = 0)
+                    long out_stride, cudaStream_t st, int stream0 = 0, const StreamRef* slots = nullptr)
 {
+  float* const state0 = slots ? m->d_state : m->d_state + (size_t)stream0 * (size_t)m->state_stride;
   if (m->use_generic && m->gen_spec_kernel != nullptr && m->opts.kernel_geometry == 0)
   {
-    GenSpecKernelParams sp{m->d_state + (size_t)stream0 * (size_t)m->state_stride, m->state_stride, d_in, d_out, in_stride, out_stride,
-                           batch, n_frames, m->t_base};
+    GenSpecKernelParams sp{state0, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, m->t_base, slots};
     void* args[] = {&sp};
     CUDA_CHECK(cudaLaunchKernel((const void*)m->gen_spec_kernel, dim3(std::max(1, std::min(batch, 16 * m->sm_count))), dim3(kGenTile),
                                 args, 0, st));
@@ -1124,7 +1167,8 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
     gp.net = m->gplan.net;
     gp.cond = m->gplan.cond;
     gp.has_cond = m->gplan.has_cond ? 1 : 0;
-    gp.state = m->d_state + (size_t)stream0 * (size_t)m->state_stride;
+    gp.state = state0;
+    gp.slots = slots;
     gp.state_stride = m->state_stride;
     gp.in = d_in;
     gp.out = d_out;
@@ -1138,11 +1182,12 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
     const int grid_g = std::min(batch, 16 * m->sm_count);
     if (wbytes <= 200 * 1024)
     {
-      ensure_max_dynamic_smem(reinterpret_cast<const void*>(wavenet_generic_kernel<true>), m->device, 200 * 1024);
-      wavenet_generic_kernel<true><<<grid_g, kGenTile, wbytes, st>>>(gp);
+      auto kern = slots ? wavenet_generic_kernel<true, true> : wavenet_generic_kernel<true>;
+      ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
+      kern<<<grid_g, kGenTile, wbytes, st>>>(gp);
     }
     else
-      wavenet_generic_kernel<false><<<grid_g, kGenTile, 0, st>>>(gp);
+      (slots ? wavenet_generic_kernel<false, true> : wavenet_generic_kernel<false>)<<<grid_g, kGenTile, 0, st>>>(gp);
     CUDA_CHECK(cudaGetLastError());
     m->launches++;
     return;
@@ -1151,8 +1196,9 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   WaveNetKernelParams kp{};
   kp.weights = m->d_weights;
   kp.n_weight_floats = (int)plan.blob.size();
-  kp.state = m->d_state + (size_t)stream0 * (size_t)m->state_stride;
+  kp.state = state0;
   kp.state_stride = m->state_stride;
+  kp.slots = slots;
   kp.in = d_in;
   kp.out = d_out;
   kp.in_stride = in_stride;
@@ -1209,7 +1255,7 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
         break; // the smallest variant that holds the call, or none
       {
         SpecKernelParams sp{kp.state, kp.state_stride, kp.in,  kp.out, kp.in_stride, kp.out_stride,
-                            kp.batch, kp.n_frames,     kp.t_base, nullptr, 0};
+                            kp.batch, kp.n_frames,     kp.t_base, nullptr, 0, kp.slots};
         void* args[] = {&sp};
         const int grid_s = std::max(1, std::min((batch + sv.q - 1) / sv.q, sv.ctas_per_sm * m->sm_count));
         CUDA_CHECK(cudaLaunchKernel((const void*)sv.kernel, dim3(grid_s), dim3(sv.fq * sv.q), args, sv.smem, st));
@@ -1303,7 +1349,8 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
       return;
     }
   }
-  if (m->spec_state == 1 && m->opts.kernel_geometry == 0)
+  // (the stream-pair variant, S = 2, takes no slot table: such calls run the fused kernel below)
+  if (m->spec_state == 1 && m->opts.kernel_geometry == 0 && !(slots && m->spec_geom.s == 2))
   {
     launch_wavenet_spec(m, kp, st);
     m->launches++;
@@ -1325,6 +1372,7 @@ struct LstmSpecKernelParams // mirror of namb200_lstm_spec::LstmSpecParams
   float* out;
   long in_stride, out_stride;
   int batch, n_frames;
+  const StreamRef* slots;
 };
 
 void setup_lstm_spec_kernel(nam_b200_model* m)
@@ -1401,13 +1449,13 @@ void setup_generic_spec_kernel(nam_b200_model* m)
 // `state`: rows of per-stream state to run on (nullptr = the handle's d_state; nam_b200_reset_streams prewarms a gathered
 // subset of streams in scratch rows)
 void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                 long out_stride, cudaStream_t st, float* state = nullptr)
+                 long out_stride, cudaStream_t st, float* state = nullptr, const StreamRef* slots = nullptr)
 {
   if (!state)
     state = m->d_state;
   if (m->spec_state == 1)
   {
-    LstmSpecKernelParams sp{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames};
+    LstmSpecKernelParams sp{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, slots};
     void* args[] = {&sp};
     // The step rate is bound by one warp's instruction stream as long as every warp has a scheduler to itself: four
     // lanes per stream (gate-split, 8 streams per warp: a shorter dependent chain per step) while every warp still gets a
@@ -1442,6 +1490,7 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   kp.fast_tanh = m->fast_tanh_runtime;
   kp.in_ch = m->spec.in_channels;
   kp.out_ch = m->spec.out_channels;
+  kp.slots = slots;
   const int H = ls.hidden;
   if (H <= kLstmGroupMaxHidden && ls.num_layers <= kLstmGroupMaxLayers && kp.in_ch == 1 && kp.out_ch == 1)
   {
@@ -1486,8 +1535,10 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   m->launches++;
 }
 
+// `slots` (with m->h_slots, its host copy): each listed stream reads the buffer its history is in and the update writes the
+// other one -- no global swap, so streams left out keep theirs
 void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                   long out_stride, cudaStream_t st)
+                   long out_stride, cudaStream_t st, const StreamRef* slots = nullptr)
 {
   const LinearSpec& li = m->spec.linear;
   LinearKernelParams kp{};
@@ -1502,6 +1553,8 @@ void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch
   kp.out_stride = out_stride;
   kp.batch = batch;
   kp.n_frames = n_frames;
+  kp.slots = slots;
+  kp.state_alt = m->d_state_tmp;
   const size_t smem = (((size_t)li.receptive_field + 3) & ~(size_t)3) * 4 + ((size_t)li.receptive_field - 1 + kLinThreads) * 4;
   ensure_max_dynamic_smem(reinterpret_cast<const void*>(linear_kernel), m->device, 227 * 1024);
   if (smem > 227 * 1024)
@@ -1519,6 +1572,12 @@ void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch
     linear_update_state_kernel<<<g2, 256, 0, st>>>(kp, m->d_state_tmp);
     CUDA_CHECK(cudaGetLastError());
     m->launches++;
+    if (slots)
+    {
+      for (int b = 0; b < batch; b++)
+        m->stream_flips[(size_t)m->h_slots[(size_t)b].stream]++; // (only the parity against lin_flips matters)
+      return;
+    }
     std::swap(m->d_state, m->d_state_tmp);
     // streams [batch, max_batch) keep their history in the buffer they were last written to
     m->lin_flips++;
@@ -1540,7 +1599,7 @@ int wavenet_chunk_streams(nam_b200_model* m)
 }
 
 void launch_convnet(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                    long out_stride, cudaStream_t st)
+                    long out_stride, cudaStream_t st, const StreamRef* slots = nullptr)
 {
   ConvNetKernelParams kp{};
   kp.weights = m->d_weights;
@@ -1555,36 +1614,113 @@ void launch_convnet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   kp.n_frames = n_frames;
   kp.t_base = m->t_base;
   kp.n_weight_floats = (int)((m->n_weight_floats + 3) & ~(size_t)3);
+  kp.slots = slots;
   const size_t wbytes = (size_t)kp.n_weight_floats * sizeof(float);
   const int grid = std::min(batch, 16 * m->sm_count);
   if (wbytes <= 200 * 1024)
   {
-    ensure_max_dynamic_smem(reinterpret_cast<const void*>(convnet_kernel<true>), m->device, 200 * 1024);
-    convnet_kernel<true><<<grid, kGenTile, wbytes, st>>>(kp);
+    auto kern = slots ? convnet_kernel<true, true> : convnet_kernel<true>;
+    ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
+    kern<<<grid, kGenTile, wbytes, st>>>(kp);
   }
   else
-    convnet_kernel<false><<<grid, kGenTile, 0, st>>>(kp);
+    (slots ? convnet_kernel<false, true> : convnet_kernel<false>)<<<grid, kGenTile, 0, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
 }
 
-// Run the hot path on device buffers and advance the stream clock.
-void run_device(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                long out_stride, cudaStream_t st)
+// ---- per-stream clocks and slot tables ----------------------------------------------------------------------------------
+// Does where stream s's history ends matter to the next call over it?  WaveNet / ConvNet rings are addressed by the clock;
+// Linear's flat history has no clock but lives in one buffer of a double buffer; an LSTM's h, c are just its state.
+bool phase_matters(const nam_b200_model* m)
 {
+  return m->spec.arch == Arch::WaveNet || m->spec.arch == Arch::ConvNet
+         || (m->spec.arch == Arch::Linear && m->spec.linear.receptive_field > 1);
+}
+bool in_phase(const nam_b200_model* m, size_t s)
+{
+  if (m->spec.arch == Arch::Linear)
+    return m->spec.linear.receptive_field <= 1 || ((m->lin_flips - m->stream_flips[s]) & 1u) == 0;
+  return !phase_matters(m) || m->stream_clock[s] == m->t_base;
+}
+void recount_phase(nam_b200_model* m)
+{
+  int n = 0;
+  for (size_t s = 0; s < m->stream_clock.size(); s++)
+    n += in_phase(m, s) ? 0 : 1;
+  m->n_out_of_phase = n;
+}
+// Must a contiguous call over streams [0, batch) carry an identity slot table (one of them sat out calls)?  O(1) while every
+// stream is in phase (a handle that always runs all its streams).
+bool prefix_needs_table(const nam_b200_model* m, int batch)
+{
+  if (m->n_out_of_phase == 0)
+    return false;
+  for (int b = 0; b < batch; b++)
+    if (!in_phase(m, (size_t)b))
+      return true;
+  return false;
+}
+
+// The call's slot table (streams[i], or i when streams == nullptr) -> m->h_slots -> the device table, ordered on `st` before
+// the launches that read it.  The host copy is pageable: cudaMemcpyAsync stages it before returning, so the next call may
+// rebuild it at once.  The device table waits for the previous table call's launches (slots_free).
+const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t st)
+{
+  const bool linear = m->spec.arch == Arch::Linear;
+  for (int i = 0; i < n; i++)
+  {
+    const int32_t s = streams ? streams[i] : i;
+    m->h_slots[(size_t)i] =
+      StreamRef{s, m->stream_clock[(size_t)s], (linear && ((m->lin_flips - m->stream_flips[(size_t)s]) & 1u)) ? 1 : 0, 0};
+  }
+  if (m->slots_used)
+    CUDA_CHECK(cudaStreamWaitEvent(st, m->slots_free, 0));
+  CUDA_CHECK(cudaMemcpyAsync(m->d_slots, m->h_slots.data(), (size_t)n * sizeof(StreamRef), cudaMemcpyHostToDevice, st));
+  return m->d_slots;
+}
+
+// After the launches of a table call on `st`: the listed streams' histories (and the handle's clock) moved on by n_frames
+void finish_table_call(nam_b200_model* m, int n, int n_frames, cudaStream_t st)
+{
+  CUDA_CHECK(cudaEventRecord(m->slots_free, st));
+  m->slots_used = true;
+  m->t_base += (uint32_t)n_frames;
+  for (int i = 0; i < n; i++)
+    m->stream_clock[(size_t)m->h_slots[(size_t)i].stream] += (uint32_t)n_frames;
+  m->streams_identical = false;
+  recount_phase(m);
+}
+
+// After a contiguous call without a table over [0, batch): those streams end at the new t_base, the others fell behind
+void finish_contiguous_call(nam_b200_model* m, int batch, int n_frames)
+{
+  m->t_base += (uint32_t)n_frames;
+  std::fill(m->stream_clock.begin(), m->stream_clock.begin() + batch, m->t_base);
+  m->n_out_of_phase = phase_matters(m) ? m->opts.max_batch - batch : 0;
+  m->streams_identical = false; // (prewarm() restores the flag: it feeds every stream the same zeros)
+}
+
+// Run the hot path on device buffers and advance the stream clocks.  `streams` (n = batch entries): the call's positions
+// run these streams, each from its own clock.  nullptr: streams [0, batch) -- launched without a table while all of them
+// are in phase, else with the identity table (a stream that sat out calls continues from its own clock).
+void run_device(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
+                long out_stride, cudaStream_t st, const int32_t* streams = nullptr)
+{
+  const bool table = streams != nullptr || prefix_needs_table(m, batch);
+  const StreamRef* slots = table ? upload_slots(m, streams, batch, st) : nullptr;
   switch (m->spec.arch)
   {
-    case Arch::WaveNet: launch_wavenet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st); break;
-    case Arch::LSTM: launch_lstm(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st); break;
-    case Arch::Linear: launch_linear(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st); break;
-    case Arch::ConvNet: launch_convnet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st); break;
+    case Arch::WaveNet: launch_wavenet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, 0, slots); break;
+    case Arch::LSTM: launch_lstm(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, nullptr, slots); break;
+    case Arch::Linear: launch_linear(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, slots); break;
+    case Arch::ConvNet: launch_convnet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, slots); break;
     default: throw std::runtime_error("no kernel for this architecture");
   }
-  m->t_base += (uint32_t)n_frames;
-  uint32_t* clock = m->stream_clock.data();
-  for (int b = 0; b < batch; b++)
-    clock[b] = m->t_base;
-  m->streams_identical = false; // (prewarm() restores the flag: it feeds every stream the same zeros)
+  if (table)
+    finish_table_call(m, batch, n_frames, st);
+  else
+    finish_contiguous_call(m, batch, n_frames);
 }
 
 // every stream's history ends at the handle's clock (init_state, prewarm)
@@ -1592,6 +1728,7 @@ void set_all_clocks(nam_b200_model* m)
 {
   std::fill(m->stream_clock.begin(), m->stream_clock.end(), m->t_base);
   std::fill(m->stream_flips.begin(), m->stream_flips.end(), m->lin_flips);
+  m->n_out_of_phase = 0;
 }
 
 void ensure_staging(nam_b200_model* m, size_t floats)
@@ -1689,11 +1826,16 @@ void prewarm(nam_b200_model* m)
   }
   m->streams_identical = identical; // zeros into identical streams keep them identical
   if (identical)
+  {
+    // every stream now holds stream 0's state, in d_state, ending where stream 0's does
     broadcast_state(m);
-  if (m->spec.arch == Arch::Linear && m->d_state_tmp)
-    CUDA_CHECK(cudaMemcpyAsync(m->d_state_tmp, m->d_state, (size_t)m->state_stride * m->opts.max_batch * sizeof(float),
-                               cudaMemcpyDeviceToDevice, m->stream));
-  set_all_clocks(m); // (broadcast or not, every stream now ends where stream 0 does)
+    if (m->spec.arch == Arch::Linear && m->d_state_tmp)
+      CUDA_CHECK(cudaMemcpyAsync(m->d_state_tmp, m->d_state, (size_t)m->state_stride * m->opts.max_batch * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, m->stream));
+    set_all_clocks(m);
+  }
+  // (otherwise every stream ran from its own clock -- with the identity table when one of them sat out calls -- and
+  // run_device left each clock and Linear buffer where that stream's history now ends: a stream that was behind stays behind)
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 
@@ -1794,6 +1936,7 @@ void mark_written(nam_b200_model* m, const int32_t* streams, int n)
     m->stream_flips[(size_t)streams[i]] = m->lin_flips;
   }
   m->streams_identical = false; // (a later prewarm must not broadcast stream 0 over them)
+  recount_phase(m);
 }
 
 // unpack records src + i * stride (stride 0: one record for all) into streams[0..n) at the handle's clock
@@ -2051,6 +2194,9 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
       CUDA_CHECK(cudaMalloc(&m->d_state_tmp, std::max<size_t>(state_total, 4) * sizeof(float)));
     m->stream_clock.assign((size_t)m->opts.max_batch, 0u);
     m->stream_flips.assign((size_t)m->opts.max_batch, 0u);
+    m->h_slots.assign((size_t)m->opts.max_batch, StreamRef{0, 0u, 0, 0});
+    CUDA_CHECK(cudaMalloc(&m->d_slots, (size_t)m->opts.max_batch * sizeof(StreamRef)));
+    CUDA_CHECK(cudaEventCreateWithFlags(&m->slots_free, cudaEventDisableTiming));
     try
     {
       setup_state_records(m.get());
@@ -2212,14 +2358,15 @@ int check_stream_list(const nam_b200_model* m, const int32_t* idx, int n, const 
   if (n > 0 && !idx)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, std::string(what) + ": null stream list");
   std::vector<char> seen(distinct ? (size_t)m->opts.max_batch : 0, 0);
+  // (the message is only built for the failing entry: a per-call table of thousands of streams passes through here)
+  auto at = [&](int i) { return std::string(what) + "[" + std::to_string(i) + "] = " + std::to_string(idx[i]); };
   for (int i = 0; i < n; i++)
   {
     const int32_t s = idx[i];
-    const std::string at = std::string(what) + "[" + std::to_string(i) + "] = " + std::to_string(s);
     if (s < 0 || s >= m->opts.max_batch)
-      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + ": stream index outside [0, max_batch=" + std::to_string(m->opts.max_batch) + ")");
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at(i) + ": stream index outside [0, max_batch=" + std::to_string(m->opts.max_batch) + ")");
     if (distinct && seen[(size_t)s]++)
-      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + ": duplicate destination stream");
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, at(i) + ": duplicate destination stream");
   }
   return NAM_B200_OK;
 }
@@ -2261,6 +2408,101 @@ int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i
   if (h.fingerprint != want.fingerprint)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "model fingerprint " + hex[0] + " is not this model's (" + hex[1]
                                                  + "): a record of another model, or of another slimmable size");
+  return NAM_B200_OK;
+}
+
+// The host-buffer entries (nam_b200_process_f32, nam_b200_process_streams_f32): `streams` (n entries) or, when nullptr,
+// streams [0, n).  Large WaveNet batches are pipelined in chunks of whole kernel waves so that the copies of chunk c+1 /
+// c-1 overlap the kernel of chunk c (the kernel is compute-bound; the copies would otherwise add ~18 %); a chunk of a table
+// call is a sub-range of the table.  Returns once `out` is filled.
+void process_host(nam_b200_model* m, const int32_t* streams, int n, const float* in, float* out, int n_frames, int64_t in_stride,
+                  int64_t out_stride)
+{
+  const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
+  const size_t row = (size_t)n_frames * sizeof(float);
+  const int chunk = wavenet_chunk_streams(m);
+  if (chunk > 0 && n >= 2 * chunk && (size_t)n * row >= ((size_t)8 << 20))
+  {
+    const int n_chunks = (n + chunk - 1) / chunk;
+    if (!m->copy_in)
+    {
+      CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_in, cudaStreamNonBlocking));
+      CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_out, cudaStreamNonBlocking));
+    }
+    while ((int)m->chunk_events.size() < 2 * n_chunks)
+    {
+      cudaEvent_t e;
+      CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      m->chunk_events.push_back(e);
+    }
+    const bool table = streams != nullptr || prefix_needs_table(m, n);
+    CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
+    const StreamRef* slots = table ? upload_slots(m, streams, n, m->stream) : nullptr;
+    for (int c = 0; c < n_chunks; c++)
+    {
+      const int s0 = c * chunk, nb = std::min(chunk, n - s0);
+      float* din = m->d_in + (size_t)s0 * n_frames;
+      float* dout = m->d_out + (size_t)s0 * n_frames;
+      cudaEvent_t e_in = m->chunk_events[2 * c], e_k = m->chunk_events[2 * c + 1];
+      CUDA_CHECK(cudaMemcpy2DAsync(din, row, in + (size_t)s0 * in_stride, (size_t)in_stride * sizeof(float), row,
+                                   (size_t)nb, cudaMemcpyHostToDevice, m->copy_in));
+      CUDA_CHECK(cudaEventRecord(e_in, m->copy_in));
+      CUDA_CHECK(cudaStreamWaitEvent(m->stream, e_in, 0));
+      launch_wavenet(m, din, dout, nb, n_frames, n_frames, n_frames, m->stream, s0, slots ? slots + s0 : nullptr);
+      CUDA_CHECK(cudaEventRecord(e_k, m->stream));
+      CUDA_CHECK(cudaStreamWaitEvent(m->copy_out, e_k, 0));
+      CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s0 * out_stride, (size_t)out_stride * sizeof(float), dout, row, row,
+                                   (size_t)nb, cudaMemcpyDeviceToHost, m->copy_out));
+    }
+    if (table)
+      finish_table_call(m, n, n_frames, m->stream);
+    else
+      finish_contiguous_call(m, n, n_frames);
+    CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
+    CUDA_CHECK(cudaStreamSynchronize(m->copy_out));
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    m->timing_valid = true;
+    return;
+  }
+  // (multi-channel models: a stream's row is its channel planes back to back)
+  CUDA_CHECK(cudaMemcpy2DAsync(m->d_in, ci * row, in, (size_t)in_stride * sizeof(float), ci * row, (size_t)n,
+                               cudaMemcpyHostToDevice, m->stream));
+  CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
+  run_device(m, m->d_in, m->d_out, n, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream, streams);
+  CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
+  CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)out_stride * sizeof(float), m->d_out, co * row, co * row, (size_t)n,
+                               cudaMemcpyDeviceToHost, m->stream));
+  CUDA_CHECK(cudaStreamSynchronize(m->stream));
+  m->timing_valid = true;
+}
+
+// nam_b200_process_streams_f32(_device): everything checked on the host before anything is queued
+int check_process_streams_args(const nam_b200_model* m, const char* fn, const int32_t* streams, int n, const void* in,
+                               const void* out, int n_frames, int64_t in_stride, int64_t out_stride)
+{
+  const std::string f(fn);
+  if (!m->is_reset)
+    return fail(NAM_B200_ERR_STATE, f + " called before reset");
+  if (n < 0 || n > m->opts.max_batch)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT,
+                f + ": n = " + std::to_string(n) + " outside [0, max_batch=" + std::to_string(m->opts.max_batch) + "]");
+  if (n_frames < 0 || n_frames > m->max_frames)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": n_frames " + std::to_string(n_frames) + " outside [0, max_frames="
+                                                 + std::to_string(m->max_frames) + "] of the last reset");
+  if (n == 0 || n_frames == 0)
+    return NAM_B200_OK;
+  if (!in || !out)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": null audio buffer");
+  const int rc = check_stream_list(m, streams, n, (f + ": streams").c_str(), true);
+  if (rc != NAM_B200_OK)
+    return rc;
+  const int64_t ci = m->spec.in_channels, co = m->spec.out_channels;
+  if (in_stride < ci * n_frames)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": in_stride " + std::to_string(in_stride) + " < in_channels x n_frames = "
+                                                 + std::to_string(ci * n_frames));
+  if (out_stride < co * n_frames)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": out_stride " + std::to_string(out_stride)
+                                                 + " < out_channels x n_frames = " + std::to_string(co * n_frames));
   return NAM_B200_OK;
 }
 
@@ -2767,6 +3009,7 @@ int nam_b200_copy_streams(nam_b200_model* m, const int32_t* src, const int32_t* 
       m->stream_flips[(size_t)dst[i]] = flips[(size_t)i];
     }
     m->streams_identical = false;
+    recount_phase(m);
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return NAM_B200_OK;
   });
@@ -2932,59 +3175,38 @@ int nam_b200_process_f32(nam_b200_model* m, const float* in, float* out, int bat
     const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
     if ((size_t)in_stride < ci * n_frames || (size_t)out_stride < co * n_frames)
       return fail(NAM_B200_ERR_INVALID_ARGUMENT, "stride smaller than channels x n_frames");
-    const size_t row = (size_t)n_frames * sizeof(float);
-    // Large WaveNet batches: pipeline the call in chunks of whole kernel waves so that the copies of chunk c+1 /
-    // c-1 overlap the kernel of chunk c (the kernel is compute-bound; the copies would otherwise add ~18 %).
-    const int chunk = wavenet_chunk_streams(m);
-    if (chunk > 0 && batch >= 2 * chunk && (size_t)batch * row >= ((size_t)8 << 20))
-    {
-      const int n_chunks = (batch + chunk - 1) / chunk;
-      if (!m->copy_in)
-      {
-        CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_in, cudaStreamNonBlocking));
-        CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_out, cudaStreamNonBlocking));
-      }
-      while ((int)m->chunk_events.size() < 2 * n_chunks)
-      {
-        cudaEvent_t e;
-        CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        m->chunk_events.push_back(e);
-      }
-      CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-      for (int c = 0; c < n_chunks; c++)
-      {
-        const int s0 = c * chunk, nb = std::min(chunk, batch - s0);
-        float* din = m->d_in + (size_t)s0 * n_frames;
-        float* dout = m->d_out + (size_t)s0 * n_frames;
-        cudaEvent_t e_in = m->chunk_events[2 * c], e_k = m->chunk_events[2 * c + 1];
-        CUDA_CHECK(cudaMemcpy2DAsync(din, row, in + (size_t)s0 * in_stride, (size_t)in_stride * sizeof(float), row,
-                                     (size_t)nb, cudaMemcpyHostToDevice, m->copy_in));
-        CUDA_CHECK(cudaEventRecord(e_in, m->copy_in));
-        CUDA_CHECK(cudaStreamWaitEvent(m->stream, e_in, 0));
-        launch_wavenet(m, din, dout, nb, n_frames, n_frames, n_frames, m->stream, s0);
-        CUDA_CHECK(cudaEventRecord(e_k, m->stream));
-        CUDA_CHECK(cudaStreamWaitEvent(m->copy_out, e_k, 0));
-        CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s0 * out_stride, (size_t)out_stride * sizeof(float), dout, row, row,
-                                     (size_t)nb, cudaMemcpyDeviceToHost, m->copy_out));
-      }
-      m->t_base += (uint32_t)n_frames;
-      std::fill(m->stream_clock.begin(), m->stream_clock.begin() + batch, m->t_base);
-      m->streams_identical = false;
-      CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
-      CUDA_CHECK(cudaStreamSynchronize(m->copy_out));
-      CUDA_CHECK(cudaStreamSynchronize(m->stream));
-      m->timing_valid = true;
-      return NAM_B200_OK;
-    }
-    // (multi-channel models: a stream's row is its channel planes back to back)
-    CUDA_CHECK(cudaMemcpy2DAsync(m->d_in, ci * row, in, (size_t)in_stride * sizeof(float), ci * row, (size_t)batch,
-                                 cudaMemcpyHostToDevice, m->stream));
-    CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-    run_device(m, m->d_in, m->d_out, batch, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream);
-    CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
-    CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)out_stride * sizeof(float), m->d_out, co * row, co * row, (size_t)batch,
-                                 cudaMemcpyDeviceToHost, m->stream));
-    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    process_host(m, nullptr, batch, in, out, n_frames, in_stride, out_stride);
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_process_streams_f32(nam_b200_model* m, const int32_t* streams, int n, const float* in, float* out, int n_frames,
+                                 int64_t in_stride, int64_t out_stride)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    const int rc = check_process_streams_args(m, "process_streams_f32", streams, n, in, out, n_frames, in_stride, out_stride);
+    if (rc != NAM_B200_OK || n == 0 || n_frames == 0)
+      return rc;
+    process_host(m, streams, n, in, out, n_frames, in_stride, out_stride);
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_process_streams_f32_device(nam_b200_model* m, const int32_t* streams, int n, const float* in_device,
+                                        float* out_device, int n_frames, int64_t in_stride, int64_t out_stride,
+                                        void* cuda_stream)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    const int rc =
+      check_process_streams_args(m, "process_streams_f32_device", streams, n, in_device, out_device, n_frames, in_stride, out_stride);
+    if (rc != NAM_B200_OK || n == 0 || n_frames == 0)
+      return rc;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
+    CUDA_CHECK(cudaEventRecord(m->ev0, st));
+    run_device(m, in_device, out_device, n, n_frames, (long)in_stride, (long)out_stride, st, streams);
+    CUDA_CHECK(cudaEventRecord(m->ev1, st));
     m->timing_valid = true;
     return NAM_B200_OK;
   });

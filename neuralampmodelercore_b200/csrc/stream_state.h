@@ -80,14 +80,8 @@ struct StateChunk
   int seg, item0;
 };
 
-// one stream of a pack / unpack launch
-struct StreamRef
-{
-  int32_t stream;
-  uint32_t clock; // the handle clock at which the stream's history ends (pack) or will end (unpack)
-  int32_t alt; // pack only: read the stream from the alternate buffer (Linear's double buffer)
-  int32_t pad;
-};
+// one stream of a pack / unpack launch: StreamRef (generic_desc.h); `alt` is read by pack only
+static_assert(sizeof(StreamRef) == 16, "StreamRef is 16 bytes");
 
 constexpr int kStateThreads = 256;
 

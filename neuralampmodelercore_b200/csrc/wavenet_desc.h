@@ -4,6 +4,8 @@
 
 #include <stdint.h>
 
+#include "generic_desc.h" // StreamRef
+
 namespace namb200
 {
 
@@ -85,6 +87,9 @@ struct WaveNetKernelParams
   // call's outputs are visible to the host (nullptr: none)
   unsigned* done_flag;
   unsigned done_seq;
+  // slot table (nullptr: position b of the call is state row b, its history ending at t_base): position b uses state row
+  // slots[b].stream, whose history ends at slots[b].clock.  Inputs, outputs, hist and tile flags stay indexed by position.
+  const StreamRef* slots;
 };
 
 } // namespace namb200

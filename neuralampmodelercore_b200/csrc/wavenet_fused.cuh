@@ -305,11 +305,14 @@ __device__ __forceinline__ void axpy_row(u64 (&acc)[C / 2], const float* __restr
 //          short calls (the reference tools' 64-frame blocks) are latency-bound per stream (20 layers x 2
 //          barriers x ring loads), so several streams walk the layer chain together and share the weights.
 //   state[j], Tv[j]: ring base and number of valid frames of the stream that owns this thread's j-th frame
-//          (Tv[j] == 0 for a slot beyond the batch); state0 / stream0 / n_streams locate the other sub-tiles' rings
-//          for the halo fill.
+//          (Tv[j] == 0 for a slot beyond the batch); stream0 locates the other sub-tiles' rings for the halo fill.
+//   tabs0: absolute ring column of the tile's first frame, t_base + t0.  With a slot table (TBL) every stream's columns
+//          are addressed from its own clock instead (WaveNetKernelParams::slots), re-read where they are used: the
+//          streams of a tile need not share one.
 //   LS   : lock-step tile-parallel mode (Q == 1 only): hist_a = this stream's history buffer at the array's first
 //          plane, t0 = call-relative first frame of the tile (see WaveNetKernelParams::hist)
-template <int CIN, int C, int HOUT, int S, int NT, int LQ, bool LS>
+//   TBL  : the call carries a slot table (WaveNetKernelParams::slots); false compiles the table out entirely
+template <int CIN, int C, int HOUT, int S, int NT, int LQ, bool LS, bool TBL>
 __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, const ArrayDesc& A,
                                               const float* __restrict__ sw, float4* __restrict__ tile,
                                               float* const (&state)[S], const int stream0, const uint32_t tabs0,
@@ -341,7 +344,20 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
   const int f_warp = (tid & (FQ - 1)) & ~31; // first frame of this warp inside its sub-tile (same for every j)
   auto sub_state = [&](int q) -> float* {
     const int s = min(stream0 + q, p.batch - 1);
-    return p.state + (size_t)s * p.state_stride;
+    return p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
+  };
+  // absolute ring column of frame t0 of sub-tile q's stream, and of the stream of this thread's j-th frame
+  // (without a table both are tabs0: the table-free instantiation is the code of a handle-wide clock)
+  auto sub_tabs = [&](int q) -> uint32_t {
+    if constexpr (!TBL)
+      return tabs0;
+    const int s = min(stream0 + q, p.batch - 1);
+    return p.slots[s].clock + (uint32_t)t0;
+  };
+  auto tabs_j = [&](int j) -> uint32_t {
+    if constexpr (!TBL)
+      return tabs0;
+    return sub_tabs(Q == 1 ? 0 : (j * NT + tid) >> LQ);
   };
 
   // ---- rechannel (Conv1x1, no bias; model.cpp:492) -> this thread's columns of the tile
@@ -404,7 +420,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
         const int pl = idx / halo, col = idx - pl * halo;
         const int a = t0 - halo + col;
         tile[pl * TW + kHalo - halo + col] = ld_ring(
-          a >= 0 ? hist_l + (size_t)pl * NC + a : ring[0] + pl * R + ((tabs0 - (uint32_t)halo + (uint32_t)col) & ring_mask));
+          a >= 0 ? hist_l + (size_t)pl * NC + a : ring[0] + pl * R + ((sub_tabs(0) - (uint32_t)halo + (uint32_t)col) & ring_mask));
       }
     }
     else if constexpr (Q == 1)
@@ -413,7 +429,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
       {
         const int pl = idx / halo, col = idx - pl * halo;
         tile[pl * TW + kHalo - halo + col] =
-          ld_ring(ring[0] + pl * R + ((tabs0 - (uint32_t)halo + (uint32_t)col) & ring_mask));
+          ld_ring(ring[0] + pl * R + ((sub_tabs(0) - (uint32_t)halo + (uint32_t)col) & ring_mask));
       }
     }
     else
@@ -424,7 +440,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
         const int pl = t2 % P, q = t2 / P;
         const float4* __restrict__ rq = reinterpret_cast<const float4*>(sub_state(q) + Ld.ring_off);
         tile[pl * TW + q * SW + kHalo - halo + col] =
-          ld_ring(rq + pl * R + ((tabs0 - (uint32_t)halo + (uint32_t)col) & ring_mask));
+          ld_ring(rq + pl * R + ((sub_tabs(q) - (uint32_t)halo + (uint32_t)col) & ring_mask));
       }
     }
     if (!LS || halo > 0) // (LS: the hand-over's barrier already made the tile columns visible)
@@ -488,7 +504,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
         const int rel = fj[j] - off;
         glob[j] = rel < -halo;
         sp[j] = tile + colj[j] - off;
-        gi[j] = (tabs0 + (uint32_t)rel) & ring_mask;
+        gi[j] = (tabs_j(j) + (uint32_t)rel) & ring_mask;
         if constexpr (LS)
         {
           const bool in_call = t0 + rel >= 0;
@@ -566,7 +582,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
       {
         const float4 own = tile[pl * TW + colj[j]];
         if (keep)
-          st_ring(ring[j] + pl * R + ((tabs0 + (uint32_t)fj[j]) & ring_mask), own);
+          st_ring(ring[j] + pl * R + ((tabs_j(j) + (uint32_t)fj[j]) & ring_mask), own);
         const float4 pb = *reinterpret_cast<const float4*>(w_pb + 4 * pl);
         hn[j][2 * pl] = pack2(own.x + pb.x, own.y + pb.y);
         hn[j][2 * pl + 1] = pack2(own.z + pb.z, own.w + pb.w);
@@ -646,7 +662,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
         const int pl = idx / HL, col = idx - pl * HL;
         const int a = t0 - HL + col;
         tile[pl * TW + kHalo - HL + col] =
-          ld_ring(a >= 0 ? hist_h + (size_t)pl * NC + a : hring[0] + pl * HR + ((tabs0 - (uint32_t)HL + (uint32_t)col) & hmask));
+          ld_ring(a >= 0 ? hist_h + (size_t)pl * NC + a : hring[0] + pl * HR + ((sub_tabs(0) - (uint32_t)HL + (uint32_t)col) & hmask));
       }
     }
     else
@@ -657,7 +673,8 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
         const int pl = t2 % P, q = t2 / P;
         const float4* __restrict__ rq =
           (Q == 1) ? hring[0] : reinterpret_cast<const float4*>(sub_state(q) + A.head_ring_off);
-        tile[pl * TW + q * SW + kHalo - HL + col] = ld_ring(rq + pl * HR + ((tabs0 - (uint32_t)HL + (uint32_t)col) & hmask));
+        const uint32_t tq = sub_tabs(Q == 1 ? 0 : q);
+        tile[pl * TW + q * SW + kHalo - HL + col] = ld_ring(rq + pl * HR + ((tq - (uint32_t)HL + (uint32_t)col) & hmask));
       }
     }
     __syncthreads(); // accumulator columns + halo visible; all ring reads done before the ring is rewritten
@@ -668,7 +685,7 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
       {
 #pragma unroll
         for (int pl = 0; pl < P; pl++)
-          st_ring(hring[j] + pl * HR + ((tabs0 + (uint32_t)fj[j]) & hmask), tile[pl * TW + colj[j]]);
+          st_ring(hring[j] + pl * HR + ((tabs_j(j) + (uint32_t)fj[j]) & hmask), tile[pl * TW + colj[j]]);
       }
       float out[HOUT];
 #pragma unroll
@@ -781,7 +798,8 @@ __device__ __forceinline__ void ls_write_back(const WaveNetKernelParams& p, cons
 
 // One persistent CTA per slot of Q = (S * NT) >> LQ streams.  C1 == 0: single layer array.
 // LS: lock-step tile-parallel mode (one CTA per (stream, tile), see WaveNetKernelParams::hist); needs tile_flags.
-template <int C0, int C1, int S, int NT, int MINB, int LQ, bool LS = false>
+// TBL: the call carries a slot table (a separate instantiation, so calls without one run exactly the table-free code).
+template <int C0, int C1, int S, int NT, int MINB, int LQ, bool LS = false, bool TBL = false>
 __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_constant__ WaveNetKernelParams p)
 {
   static_assert(!LS || (S * NT) == (1 << LQ), "lock-step mode: one stream per tile");
@@ -822,6 +840,8 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
   for (int stream0 = s_begin; stream0 < s_end; stream0 += s_step)
   {
     // the stream each of this thread's frames belongs to (slots beyond the batch alias the last stream, masked by Tv)
+    // (position sc of the call: state row from the slot table, or row sc; array_forward reads the clocks)
+    auto position = [&](int j) -> int { return min(stream0 + ((Q == 1 ? 0 : j * NT + tid) >> LQ), p.batch - 1); };
     float* state[S];
     const float* xin[S];
     float* yout[S];
@@ -834,7 +854,8 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
       const int sj = stream0 + (trel >> LQ);
       live[j] = sj < p.batch;
       const size_t sc = (size_t)min(sj, p.batch - 1);
-      state[j] = p.state + sc * p.state_stride;
+      const size_t row = TBL ? (size_t)p.slots[position(j)].stream : sc;
+      state[j] = p.state + row * p.state_stride;
       xin[j] = p.in + sc * p.in_stride;
       yout[j] = p.out + sc * p.out_stride;
       fj[j] = trel & (FQ - 1);
@@ -867,7 +888,7 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
           for (int q = 0; q < C0 / 2; q++)
             head0[j][q] = 0ull; // model.cpp:469
         float hout0[S][C0], ho0[S][1];
-        array_forward<1, C0, 1, S, NT, LQ, LS>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
+        array_forward<1, C0, 1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
                                                head0, hout0, ho0);
 #pragma unroll
         for (int j = 0; j < S; j++)
@@ -883,7 +904,7 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
 #pragma unroll
             for (int q = 0; q < C0 / 2; q++)
               head0[j][q] = 0ull;
-          array_forward<1, C0, C1, S, NT, LQ, LS>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
+          array_forward<1, C0, C1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
                                                   head0, hout0, ho0);
         }
         // second array: layer input = previous array's layer output, head accumulator starts from
@@ -895,7 +916,7 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
           for (int q = 0; q < C1 / 2; q++)
             head1[j][q] = pack2(ho0[j][2 * q], ho0[j][2 * q + 1]);
         float hout1[S][C1], ho1[S][1];
-        array_forward<C0, C1, 1, S, NT, LQ, LS>(p, p.arrays[1], sw, tile, state, stream0, tabs0, ts, step1, hist1, t0, Tv, hout0,
+        array_forward<C0, C1, 1, S, NT, LQ, LS, TBL>(p, p.arrays[1], sw, tile, state, stream0, tabs0, ts, step1, hist1, t0, Tv, hout0,
                                                 cond, head1, hout1, ho1);
 #pragma unroll
         for (int j = 0; j < S; j++)
@@ -912,9 +933,10 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
         for (int k = tid; k < p.tiles_per_stream; k += NT)
           ls_spin_until_above(ts.mine - ts.tile_i + k, kLsFinalStep);
         __syncthreads();
-        ls_write_back<C0, S, NT, LQ>(p, p.arrays[0], state[0], hist0, t0, tabs0, Tv[0]);
+        const uint32_t tabs_s = TBL ? p.slots[position(0)].clock + (uint32_t)t0 : tabs0;
+        ls_write_back<C0, S, NT, LQ>(p, p.arrays[0], state[0], hist0, t0, tabs_s, Tv[0]);
         if constexpr (C1 != 0)
-          ls_write_back<C1, S, NT, LQ>(p, p.arrays[1], state[0], hist1, t0, tabs0, Tv[0]);
+          ls_write_back<C1, S, NT, LQ>(p, p.arrays[1], state[0], hist1, t0, tabs_s, Tv[0]);
       }
     }
     __syncthreads(); // the next streams reuse the tile

@@ -304,9 +304,10 @@ __device__ __forceinline__ void g_net(const GenThread& c, const GNet& N, const G
 // The C ABI's batched entry; persistent CTAs, one stream at a time.  Multi-channel models (model.cpp:809-820,
 // :888-909): stream s's channel c is the plane in[s * in_stride + c * n_frames ..] (out likewise); the input vector
 // is both the first array's layer input and -- unless a condition_dsp produces it -- the condition.
+// TBL: the call carries a slot table (its own instantiation: a call without one runs the table-free code).
 // WS: the weight blob is staged in shared memory once per CTA (it fits for every model the kernel accepts in
 // practice: example_models/wavenet_a2_max.nam is 7.5 KB); otherwise it is read through the read-only path.
-template <bool WS>
+template <bool WS, bool TBL = false>
 __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_constant__ GenericKernelParams p)
 {
   extern __shared__ float4 gen_smem4[];
@@ -323,14 +324,16 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
   const int ci = p.net.in_channels, co = p.net.out_channels;
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
-    c.st = p.state + (size_t)s * p.state_stride;
+    // position s of the call: state row and clock from the slot table, or row s at the handle's clock
+    const uint32_t clock = TBL ? p.slots[s].clock : p.t_base;
+    c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
     for (int t0 = 0; t0 < p.n_frames; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;
       c.valid = f < p.n_frames;
-      c.t = p.t_base + (uint32_t)f;
+      c.t = clock + (uint32_t)f;
       float in[kGenMaxVec], out[kGenMaxVec], cond[kGenMaxVec];
       for (int ch = 0; ch < ci; ch++)
         in[ch] = c.valid ? __ldg(xin + (size_t)ch * p.n_frames + f) : 0.0f;
@@ -349,7 +352,7 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
 
 // ConvNet (NAM/convnet.cpp:204-272): the same frame-per-thread tiling; a block is Conv1D(kernel 2, dilation d) ->
 // BatchNorm as two separate roundings, multiply then add (convnet.cpp:39-46) -> activation (:66-88); head W x + b.
-template <bool WS>
+template <bool WS, bool TBL = false>
 __global__ void __launch_bounds__(kGenTile) convnet_kernel(const __grid_constant__ ConvNetKernelParams p)
 {
   extern __shared__ float4 gen_smem4[];
@@ -366,14 +369,15 @@ __global__ void __launch_bounds__(kGenTile) convnet_kernel(const __grid_constant
   const GConvNet& N = p.net;
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
-    c.st = p.state + (size_t)s * p.state_stride;
+    const uint32_t clock = TBL ? p.slots[s].clock : p.t_base;
+    c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
     for (int t0 = 0; t0 < p.n_frames; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;
       c.valid = f < p.n_frames;
-      c.t = p.t_base + (uint32_t)f;
+      c.t = clock + (uint32_t)f;
       float x[kGenMaxVec], z[kGenMaxVec];
       for (int ch = 0; ch < N.in_channels; ch++)
         x[ch] = c.valid ? __ldg(xin + (size_t)ch * p.n_frames + f) : 0.0f;

@@ -55,6 +55,7 @@ struct LatParams
   // is visible to the host -- the host spins on it instead of paying a stream synchronisation per 64-frame call
   unsigned* done_flag;
   unsigned seq;
+  const SlotRef* slots; // as SpecParams::slots
 };
 
 // ---- shared-memory plan (float4 columns) ------------------------------------------------------------------------------
@@ -394,8 +395,8 @@ __device__ __forceinline__ void wavenet_lat_body(const LatParams& p)
   c.xbuf = lat_smem + Plan<F>::pmax() * F;
   c.win = lat_smem + 2 * Plan<F>::pmax() * F;
   c.bars = bars;
-  c.state = p.state + (size_t)stream * p.state_stride;
-  c.tabs0 = p.t_base;
+  c.state = p.state + (size_t)(p.slots ? p.slots[stream].stream : stream) * p.state_stride;
+  c.tabs0 = p.slots ? p.slots[stream].clock : p.t_base;
   c.n = p.n_frames;
   c.f = tid & (F - 1);
   const int g = tid / F; // warp-uniform: F is a multiple of 32

@@ -304,7 +304,8 @@ __device__ __forceinline__ void lat2_array(const WaveNetKernelParams& p, const A
 
 // One CTA per stream; C1 == 0: single layer array.  The completion doorbell (p.done_flag, may be null) is rung once the
 // outputs are visible to the host.
-template <int C0, int C1, int FW>
+// TBL: the call carries a slot table (its own instantiation: a call without one runs the table-free code).
+template <int C0, int C1, int FW, bool TBL = false>
 __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_constant__ WaveNetKernelParams p)
 {
   constexpr int F = 32 * FW, NTH = kLatGroups * F, NWARPS = NTH / 32;
@@ -317,8 +318,9 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   float4* const tile = lat2_smem + wf4;
   float4* const xbuf = tile + PMAX * F;
   float4* const win = xbuf + PMAX * F;
-  const int stream = blockIdx.x;
-  float* const state = p.state + (size_t)stream * p.state_stride;
+  const int stream = blockIdx.x; // position in the call (input / output row)
+  float* const state = p.state + (size_t)(TBL ? p.slots[stream].stream : stream) * p.state_stride;
+  const uint32_t clock = TBL ? p.slots[stream].clock : p.t_base; // where this stream's history ends
 
   // window table: float4 offset of each layer's first window (prefix sums, thread li computes entry li) -- it lives
   // behind the windows; total window size is bounded by the host (lat2_smem_bytes)
@@ -394,7 +396,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
         if (lane < Pa)
         {
           float4* dst = win + base + lane * wn;
-          const int start = (int)((p.t_base - (uint32_t)off) & (uint32_t)Ld.ring_mask);
+          const int start = (int)((clock - (uint32_t)off) & (uint32_t)Ld.ring_mask);
           const int n1 = min(wn, R - start);
           lat_bulk_g2s(dst, ring + lane * R + start, (uint32_t)n1 * 16u, bars + LI);
           if (n1 < wn)
@@ -413,7 +415,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   c.woff = woff;
   c.bars = bars;
   c.state = state;
-  c.tabs0 = p.t_base;
+  c.tabs0 = clock;
   c.n = p.n_frames;
   c.f = tid & (F - 1);
   c.g = tid / F;

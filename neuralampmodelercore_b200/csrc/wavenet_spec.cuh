@@ -54,6 +54,14 @@ enum : int
   ACT_SOFTSIGN = 10
 };
 
+// layout twin of namb200::StreamRef (generic_desc.h): one entry of a call's slot table
+struct SlotRef
+{
+  int stream; // state row of this position of the call
+  u32 clock; // where that row's history ends
+  int alt, pad;
+};
+
 struct SpecParams
 {
   float* state; // [batch][state_stride]: the rings of wavenet_fused.cuh
@@ -65,6 +73,9 @@ struct SpecParams
   u32 t_base; // absolute frame index of in[:, 0] (mod 2^32)
   float* scratch; // S = 2: [grid][scratch_stride] floats, a CTA's stream pair in the interleaved layout
   long scratch_stride; // 2 * state_stride
+  // slot table (nullptr: position b is state row b at t_base): position b uses row slots[b].stream at slots[b].clock; inputs
+  // and outputs stay indexed by position.  The stream-pair variant (S = 2) is never given one.
+  const SlotRef* slots;
 };
 
 // ---- scalar helpers (same arithmetic as wavenet_fused.cuh) ------------------------------------------------------
@@ -694,8 +705,10 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
   {
     const int sa = S * unit, sb = min(sa + 1, p.batch - 1);
     const bool live_b = (S == 2) && (sa + 1 < p.batch); // an odd batch leaves the last pair's second half idle
-    float* const state_a = p.state + (size_t)sa * p.state_stride;
+    const bool table = (S == 1) && p.slots != nullptr;
+    float* const state_a = p.state + (size_t)(table ? p.slots[sa].stream : sa) * p.state_stride;
     float* const state_b = p.state + (size_t)sb * p.state_stride;
+    const u32 clock_a = table ? p.slots[sa].clock : p.t_base;
     const float* xin_a = p.in + (size_t)sa * p.in_stride;
     const float* xin_b = p.in + (size_t)sb * p.in_stride;
     float* yout_a = p.out + (size_t)sa * p.out_stride;
@@ -712,7 +725,7 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
     for (int t0 = 0; t0 < p.n_frames; t0 += T)
     {
       c.tv = min(T, p.n_frames - t0);
-      c.tabs0 = p.t_base + (u32)t0;
+      c.tabs0 = clock_a + (u32)t0;
       request_layer_history<0, NT, S>(c, IntC<spec::A[0].layer0>{});
       V x[1];
       {
@@ -1023,7 +1036,8 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
     const int stream = slot * Q + q;
     const bool live = stream < p.batch;
     const int sc = min(stream, p.batch - 1);
-    float* state = p.state + (size_t)sc * p.state_stride;
+    float* state = p.state + (size_t)(p.slots ? p.slots[sc].stream : sc) * p.state_stride;
+    const u32 clock = p.slots ? p.slots[sc].clock : p.t_base; // per q: the streams of a CTA need not share a clock
     const float xv = (live && f < p.n_frames) ? __ldg(p.in + (size_t)sc * p.in_stride + f) : 0.0f;
     const float x[1] = {xv};
     constexpr int C0 = spec::A[0].C;
@@ -1032,7 +1046,7 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
     for (int o = 0; o < C0; o++)
       head0[o] = 0.0f;
     float y;
-    array_forward_short<0, spec::NA - 1, NT, FQ>(spec_smem, state, pol, p.t_base, p.n_frames, f, live, x, xv, head0, hout0, ho0);
+    array_forward_short<0, spec::NA - 1, NT, FQ>(spec_smem, state, pol, clock, p.n_frames, f, live, x, xv, head0, hout0, ho0);
     if constexpr (spec::NA == 1)
       y = ho0[0];
     else
@@ -1044,7 +1058,7 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
       for (int o = 0; o < C1; o++)
         head1[o] = ho0[o];
       __syncthreads(); // (the last layer's tap reads are fenced by its B1; this orders the rechannel's tile stores too)
-      array_forward_short<AI1, -1, NT, FQ>(spec_smem, state, pol, p.t_base, p.n_frames, f, live, hout0, xv, head1, hout1, ho1);
+      array_forward_short<AI1, -1, NT, FQ>(spec_smem, state, pol, clock, p.n_frames, f, live, hout0, xv, head1, hout1, ho1);
       y = ho1[0];
     }
     if (live && f < p.n_frames)

@@ -317,6 +317,48 @@ class DSP:
         if rc != 0:
             _raise(rc, self._lib)
 
+    def process_streams(self, streams, x: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Run only the listed streams (distinct, any order): row i of x belongs to streams[i], and each stream continues
+        from its own history, however many calls it sat out; unlisted streams are untouched.  x: (n, frames) float32, or
+        (n, in_channels, frames) for a multi-channel model -> out of the same layout with out_channels."""
+        s = self._streams(streams)
+        x = np.asarray(x)
+        if x.ndim == 3:
+            if x.dtype != np.float32 or x.shape[1] != self.in_channels:
+                raise TypeError(f"process_streams takes a float32 array [n, {self.in_channels}, frames]")
+            n_rows, _, n = x.shape
+            shape = (n_rows, self.out_channels, n)
+        else:
+            if x.ndim != 2 or x.dtype != np.float32:
+                raise TypeError("process_streams takes a 2-D float32 array [n, frames]")
+            if self.in_channels != 1 or self.out_channels != 1:
+                raise TypeError("multi-channel model: process_streams takes [n, in_channels, frames]")
+            n_rows, n = x.shape
+            shape = (n_rows, n)
+        if n_rows != len(s):
+            raise ValueError(f"x has {n_rows} rows for {len(s)} streams")
+        x = np.ascontiguousarray(x)
+        if out is None:
+            out = np.empty(shape, np.float32)
+        elif (not isinstance(out, np.ndarray) or out.dtype != np.float32 or out.shape != shape
+              or not out.flags["C_CONTIGUOUS"]):
+            raise ValueError(f"out must be a C-contiguous float32 array of shape {shape}")
+        self._check(self._lib.nam_b200_process_streams_f32(self._h, self._i32p(s), len(s), x.ctypes.data_as(C.c_void_p),
+                                                           out.ctypes.data_as(C.c_void_p), n, self.in_channels * n,
+                                                           self.out_channels * n))
+        return out
+
+    def process_streams_device(self, streams, in_ptr: int, out_ptr: int, n_frames: int, in_stride: int | None = None,
+                               out_stride: int | None = None, cuda_stream: int = 0) -> None:
+        """process_streams on device buffers (e.g. torch.Tensor.data_ptr()), asynchronous on `cuda_stream` (0 = the
+        handle's stream).  Strides in floats between rows, default channels x n_frames."""
+        s = self._streams(streams)
+        self._check(self._lib.nam_b200_process_streams_f32_device(
+            self._h, self._i32p(s), len(s), C.c_void_p(in_ptr), C.c_void_p(out_ptr), int(n_frames),
+            int(in_stride if in_stride is not None else self.in_channels * n_frames),
+            int(out_stride if out_stride is not None else self.out_channels * n_frames),
+            C.c_void_p(cuda_stream) if cuda_stream else None))
+
     # ---- per-stream state (include/nam_b200.h: records, per-stream clocks) ------------------------------------------
     @property
     def state_record_bytes(self) -> int:
