@@ -132,7 +132,8 @@ int nam_b200_prewarm(nam_b200_model* m);
  * record carries: a record taken at one slimmable size is refused at another.
  *
  * The handle keeps, per stream, the clock value at which the stream's history ends.  A stream left out of process calls
- * (batch < max_batch, or not listed in nam_b200_process_streams_f32) keeps its history at that older point: export reads it
+ * (batch < max_batch, not listed in nam_b200_process_streams_f32, or given fewer frames than the longest row of a ragged
+ * call) keeps its history at that older point: export reads it
  * there, and every process call that includes it again continues from its own clock -- a pause needs no export, import or
  * reset.  (Contiguous calls launch exactly as before while every stream in [0, batch) is in step with the handle; otherwise
  * they carry the per-stream clocks like nam_b200_process_streams_f32.)
@@ -192,6 +193,29 @@ int nam_b200_process_streams_f32(nam_b200_model* m, const int32_t* streams, int 
 int nam_b200_process_streams_f32_device(nam_b200_model* m, const int32_t* streams, int n, const float* in_device,
                                         float* out_device, int n_frames, int64_t in_stride, int64_t out_stride,
                                         void* cuda_stream);
+
+/* Ragged calls: like nam_b200_process_streams_f32, but row i runs its own number of frames, n_frames[i], in one launch.
+ *   Layout: let n_max = max_i n_frames[i].  Row i belongs to streams[i]; channel c of row i is at
+ *     in + i*in_stride + c*n_max, its valid frames are [0, n_frames[i]) and [n_frames[i], n_max) is padding -- a
+ *     [n, channels, n_max] array maps directly.  `out` follows the same layout.  in_stride >= in_channels*n_max and
+ *     out_stride >= out_channels*n_max.
+ *   Padding: input padding is never read (NaN there changes nothing).  The device entry never writes output padding;
+ *     the host entry writes zeros there, and its host buffers must span full rows, as for a nam_b200_process_streams_f32
+ *     call of n_max frames.
+ *   State and clocks: each listed stream continues from its own clock and advances by its own n_frames[i]; the handle's
+ *     clock advances by n_max.  An entry of 0 is accepted: that stream's state and clock stay exactly as they were, the
+ *     device entry does not touch its output row and the host entry zeros it.
+ *   Checks: everything is checked on the host before anything is queued, as for nam_b200_process_streams_f32; in
+ *     addition n_frames must not be NULL when n > 0 and each entry must lie in [0, max_frames] of the last reset (a
+ *     refusal names the entry).  n == 0 or n_max == 0 does nothing.
+ *   The kernel is the one a contiguous call of batch = n and n_frames = n_max would get; nam_b200_process_streams_f32 is
+ *   this call with every count equal.  `streams` and `n_frames` are host arrays, reusable as soon as the call returns. */
+int nam_b200_process_streams_ragged_f32(nam_b200_model* m, const int32_t* streams, int n, const int32_t* n_frames,
+                                        const float* in, float* out, int64_t in_stride, int64_t out_stride);
+/* The same on device audio buffers, asynchronous on cuda_stream (NULL = the handle's stream). */
+int nam_b200_process_streams_ragged_f32_device(nam_b200_model* m, const int32_t* streams, int n, const int32_t* n_frames,
+                                               const float* in_device, float* out_device, int64_t in_stride,
+                                               int64_t out_stride, void* cuda_stream);
 
 /* Host-buffer contract of nam_b200_process_f32: any host memory is accepted; with PAGE-LOCKED buffers (cudaMallocHost,
  * cudaHostRegister, or nam_b200_pin_host_buffer below) the call pipelines host->device copy, kernel and device->host copy

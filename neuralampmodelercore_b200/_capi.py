@@ -103,6 +103,8 @@ EXPORTED_SYMBOLS = [
     "nam_b200_state_layout_json",
     "nam_b200_process_streams_f32",
     "nam_b200_process_streams_f32_device",
+    "nam_b200_process_streams_ragged_f32",
+    "nam_b200_process_streams_ragged_f32_device",
 ]
 
 
@@ -189,9 +191,12 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_state_layout_json.argtypes = [C.c_char_p, C.c_char_p, C.c_int64]
     lib.nam_b200_process_streams_f32.argtypes = [vp, i32p, C.c_int, vp, vp, C.c_int, C.c_int64, C.c_int64]
     lib.nam_b200_process_streams_f32_device.argtypes = [vp, i32p, C.c_int, vp, vp, C.c_int, C.c_int64, C.c_int64, vp]
+    lib.nam_b200_process_streams_ragged_f32.argtypes = [vp, i32p, C.c_int, i32p, vp, vp, C.c_int64, C.c_int64]
+    lib.nam_b200_process_streams_ragged_f32_device.argtypes = [vp, i32p, C.c_int, i32p, vp, vp, C.c_int64, C.c_int64, vp]
     for name in ("nam_b200_reset_streams", "nam_b200_copy_streams", "nam_b200_export_streams", "nam_b200_import_streams",
                  "nam_b200_export_streams_device", "nam_b200_import_streams_device", "nam_b200_state_layout_json",
-                 "nam_b200_process_streams_f32", "nam_b200_process_streams_f32_device"):
+                 "nam_b200_process_streams_f32", "nam_b200_process_streams_f32_device",
+                 "nam_b200_process_streams_ragged_f32", "nam_b200_process_streams_ragged_f32_device"):
         getattr(lib, name).restype = C.c_int
     for name in (
         "nam_b200_create_from_file",

@@ -86,20 +86,32 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
   __syncthreads();
 
   const int stream0 = blockIdx.x * SPC;
-  for (int t0 = 0; t0 < p.n_frames; t0 += kLstmGroupChunk)
+  // frames of the CTA's slot s (slot table: the stream's own count; 0 beyond the batch).  The chunk loop below holds
+  // barriers and the groups' shuffles, so it runs to the CTA's longest stream; a group whose stream has ended steps
+  // without keeping (c, h).
+  auto frames_of = [&](int s) -> int {
+    const int b = stream0 + s;
+    return b >= p.batch ? 0 : p.slots ? p.slots[b].frames : p.n_frames;
+  };
+  int n_cta = 0;
+  for (int s = 0; s < SPC; s++)
+    n_cta = max(n_cta, frames_of(s));
+  const int n_me = frames_of(sl);
+  for (int t0 = 0; t0 < n_cta; t0 += kLstmGroupChunk)
   {
-    const int tc = min(kLstmGroupChunk, p.n_frames - t0);
+    const int tc = min(kLstmGroupChunk, n_cta - t0);
     for (int idx = tid; idx < SPC * kLstmGroupChunk; idx += kLstmGroupThreads)
     {
       const int s = idx / kLstmGroupChunk, f = idx - s * kLstmGroupChunk;
       float v = 0.0f;
-      if (stream0 + s < p.batch && f < tc)
+      if (t0 + f < frames_of(s))
         v = __ldg(p.in + (size_t)(stream0 + s) * p.in_stride + t0 + f);
       sio[s * (kLstmGroupChunk + 1) + f] = v;
     }
     __syncthreads();
     for (int f = 0; f < tc; f++)
     {
+      const bool step = t0 + f < n_me; // false: this group's stream has ended, its (c, h) stay as they are
       const float x = sio[sl * (kLstmGroupChunk + 1) + f];
       const float* w = sw;
       float hl[UPL] = {}; // the last layer's new h
@@ -154,8 +166,9 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
           const float gi = acc[k][0] + b[unit[k]], gf = acc[k][1] + b[H + unit[k]];
           const float gg = acc[k][2] + b[2 * H + unit[k]], go = acc[k][3] + b[3 * H + unit[k]];
           const float cn = lstm_sigmoid(gf, p.fast_tanh) * c[l][k] + lstm_sigmoid(gi, p.fast_tanh) * lstm_tanh(gg, p.fast_tanh);
-          c[l][k] = cn;
-          h[l][k] = lstm_sigmoid(go, p.fast_tanh) * lstm_tanh(cn, p.fast_tanh);
+          const float hn = lstm_sigmoid(go, p.fast_tanh) * lstm_tanh(cn, p.fast_tanh);
+          c[l][k] = step ? cn : c[l][k];
+          h[l][k] = step ? hn : h[l][k];
           if (l == L - 1)
             hl[k] = h[l][k];
         }
@@ -175,7 +188,7 @@ __global__ void __launch_bounds__(kLstmGroupThreads) lstm_group_kernel(const Lst
     for (int idx = tid; idx < SPC * kLstmGroupChunk; idx += kLstmGroupThreads)
     {
       const int s = idx / kLstmGroupChunk, f = idx - s * kLstmGroupChunk;
-      if (stream0 + s < p.batch && f < tc)
+      if (t0 + f < frames_of(s))
         p.out[(size_t)(stream0 + s) * p.out_stride + t0 + f] = sout[s * (kLstmGroupChunk + 1) + f];
     }
     __syncthreads();

@@ -29,7 +29,8 @@ struct SlotRef
 {
   int stream;
   unsigned clock;
-  int alt, pad;
+  int alt;
+  int frames; // frames position b runs, <= n_frames
 };
 
 struct LstmSpecParams
@@ -40,10 +41,18 @@ struct LstmSpecParams
   float* out;
   long in_stride, out_stride;
   int batch, n_frames;
-  // slot table (nullptr: position b is state row b): position b uses row slots[b].stream; inputs and outputs stay
-  // indexed by position
+  // slot table (nullptr: position b is state row b and runs n_frames frames): position b uses row slots[b].stream and
+  // runs slots[b].frames frames; inputs and outputs stay indexed by position
   const SlotRef* slots;
 };
+
+// frames position `stream` runs (0 beyond the batch)
+__device__ __forceinline__ int position_frames(const LstmSpecParams& p, int stream)
+{
+  if (stream >= p.batch)
+    return 0;
+  return p.slots ? p.slots[stream].frames : p.n_frames;
+}
 
 __device__ __forceinline__ float rcp_approx(float x)
 {
@@ -100,6 +109,9 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
   const int stream = stream0 + lane;
   const bool live = stream < p.batch;
   const int row = p.slots ? p.slots[min(stream, p.batch - 1)].stream : min(stream, p.batch - 1); // state row
+  // frames of this lane's stream; the warp's tiles run to its longest stream, each lane's steps stop at its own count
+  const int n_me = position_frames(p, stream);
+  const int n_warp = __reduce_max_sync(0xffffffffu, n_me);
 
   float h[L][H], c[L][H];
 #pragma unroll
@@ -119,19 +131,19 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
     for (int r = 0; r < kTile; r++)
     {
       const int s = stream0 + r;
-      pre[r] = (s < p.batch && t0 + lane < p.n_frames) ? __ldg(p.in + (size_t)s * p.in_stride + t0 + lane) : 0.0f;
+      pre[r] = (t0 + lane < __shfl_sync(0xffffffffu, n_me, r)) ? __ldg(p.in + (size_t)s * p.in_stride + t0 + lane) : 0.0f;
     }
   };
   fetch(0);
-  for (int t0 = 0; t0 < p.n_frames; t0 += kTile)
+  for (int t0 = 0; t0 < n_warp; t0 += kTile)
   {
-    const int tc = min(kTile, p.n_frames - t0);
+    const int tc = min(kTile, n_me - t0); // (<= 0: this lane's stream has ended)
     __syncwarp();
 #pragma unroll
     for (int r = 0; r < kTile; r++)
       sin_[r][lane] = pre[r];
     __syncwarp();
-    if (t0 + kTile < p.n_frames)
+    if (t0 + kTile < n_warp)
       fetch(t0 + kTile);
     for (int f = 0; f < tc; f++)
     {
@@ -203,7 +215,7 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
     for (int r = 0; r < kTile; r++)
     {
       const int s = stream0 + r;
-      if (s < p.batch && lane < tc)
+      if (t0 + lane < __shfl_sync(0xffffffffu, n_me, r))
         p.out[(size_t)s * p.out_stride + t0 + lane] = sout[r][lane];
     }
   }
@@ -242,6 +254,10 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
   const bool live = stream < p.batch;
   const int row = p.slots ? p.slots[min(stream, p.batch - 1)].stream : min(stream, p.batch - 1); // state row
   const unsigned base_lane = (unsigned)(lane & ~3);
+  // frames of this group's stream.  The shuffles below need the whole warp, so every lane steps to the warp's longest
+  // stream; a group whose stream has ended computes but keeps its (c, h).
+  const int n_me = position_frames(p, stream);
+  const int n_warp = __reduce_max_sync(0xffffffffu, n_me);
 
   // my gate's rows: W[q*H + u][0 .. I+H) and b[q*H + u].  Fast regime: the 0.5 z of the sigmoid gates is folded in.
   const float sc = (FAST && q != 2) ? 0.5f : 1.0f;
@@ -287,19 +303,20 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
       c[l][u] = st[H + u];
     }
 
-  for (int t0 = 0; t0 < p.n_frames; t0 += kTile)
+  for (int t0 = 0; t0 < n_warp; t0 += kTile)
   {
-    const int tc = min(kTile, p.n_frames - t0);
+    const int tc = min(kTile, n_warp - t0);
     __syncwarp();
 #pragma unroll
     for (int r = 0; r < SPW; r++)
     {
       const int s = stream0 + r;
-      sin_[r][lane] = (s < p.batch && t0 + lane < p.n_frames) ? __ldg(p.in + (size_t)s * p.in_stride + t0 + lane) : 0.0f;
+      sin_[r][lane] = (t0 + lane < __shfl_sync(0xffffffffu, n_me, 4 * r)) ? __ldg(p.in + (size_t)s * p.in_stride + t0 + lane) : 0.0f;
     }
     __syncwarp();
     for (int f = 0; f < tc; f++)
     {
+      const bool step = t0 + f < n_me; // false: this group's stream has ended, its (c, h) stay as they are
       const float x = sin_[grp][f];
 #pragma unroll
       for (int l = 0; l < L; l++)
@@ -334,8 +351,9 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
           const float gi = __shfl_sync(0xffffffffu, g[u], base_lane + 0), gf = __shfl_sync(0xffffffffu, g[u], base_lane + 1);
           const float gg = __shfl_sync(0xffffffffu, g[u], base_lane + 2), go = __shfl_sync(0xffffffffu, g[u], base_lane + 3);
           const float cn = gf * c[l][u] + gi * gg; // lstm.cpp:50-53,61-63
-          c[l][u] = cn;
-          h[l][u] = go * tnh<FAST>(cn); // :55-57,65-66
+          const float hn = go * tnh<FAST>(cn); // :55-57,65-66
+          c[l][u] = step ? cn : c[l][u];
+          h[l][u] = step ? hn : h[l][u];
         }
       }
       // head (lstm.cpp:164-167)
@@ -352,7 +370,7 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
     for (int r = 0; r < SPW; r++)
     {
       const int s = stream0 + r;
-      if (s < p.batch && lane < tc)
+      if (t0 + lane < __shfl_sync(0xffffffffu, n_me, 4 * r))
         p.out[(size_t)s * p.out_stride + t0 + lane] = sout[r][lane];
     }
   }

@@ -133,19 +133,29 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
   __syncthreads();
 
   const int stream0 = blockIdx.x * kLstmThreads;
-  for (int t0 = 0; t0 < p.n_frames; t0 += kLstmChunk)
+  // frames of the CTA's position s (slot table: the stream's own count; 0 beyond the batch); the chunk loop holds
+  // barriers, so it runs to the CTA's longest stream
+  auto frames_of = [&](int s) -> int {
+    const int b = stream0 + s;
+    return b >= p.batch ? 0 : p.slots ? p.slots[b].frames : p.n_frames;
+  };
+  int n_cta = 0;
+  for (int s = 0; s < kLstmThreads; s++)
+    n_cta = max(n_cta, frames_of(s));
+  const int n_me = frames_of(tid);
+  for (int t0 = 0; t0 < n_cta; t0 += kLstmChunk)
   {
-    const int tc = min(kLstmChunk, p.n_frames - t0);
-    // coalesced load of the [streams x tc] input tile
+    // coalesced load of the [streams x chunk] input tile
     for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
     {
       const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
       float v = 0.0f;
-      if (stream0 + s < p.batch && f < tc)
+      if (t0 + f < frames_of(s))
         v = __ldg(p.in + (size_t)(stream0 + s) * p.in_stride + t0 + f);
       sio[s * (kLstmChunk + 1) + f] = v;
     }
     __syncthreads();
+    const int tc = min(kLstmChunk, n_me - t0); // this thread's frames in the chunk (<= 0: its stream has ended)
     if (active)
     {
       const bool multi = p.in_ch > 1 || p.out_ch > 1;
@@ -217,7 +227,7 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
     for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
     {
       const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
-      if (stream0 + s < p.batch && f < tc && p.out_ch == 1 && p.in_ch == 1)
+      if (t0 + f < frames_of(s) && p.out_ch == 1 && p.in_ch == 1)
         p.out[(size_t)(stream0 + s) * p.out_stride + t0 + f] = sout[s * (kLstmChunk + 1) + f];
     }
     __syncthreads();
@@ -270,19 +280,20 @@ __global__ void __launch_bounds__(kLinThreads) linear_kernel(const LinearKernelP
   const float* xin = p.in + (size_t)stream * p.in_stride;
   const float* st = p.slots ? (p.slots[stream].alt ? p.state_alt : p.state) + (size_t)p.slots[stream].stream * p.state_stride
                             : p.state + (size_t)stream * p.state_stride;
+  const int n = p.slots ? p.slots[stream].frames : p.n_frames; // this stream's frames
   for (int i = tid; i < hist + kLinThreads; i += kLinThreads)
   {
     const int t = t0 - hist + i; // frame index relative to this call
     float v = 0.0f;
     if (t >= 0)
-      v = (t < p.n_frames) ? __ldg(xin + t) : 0.0f;
+      v = (t < n) ? __ldg(xin + t) : 0.0f;
     else
       v = st[hist + t]; // t in [-hist, 0): state holds frames -hist..-1
     sx[i] = v;
   }
   __syncthreads();
   const int t = t0 + tid;
-  if (t < p.n_frames)
+  if (t < n)
   {
     // oldest tap first, like the reference's dot over the reversed impulse (linear.cpp:71-74,184-186)
     float acc = 0.0f;
@@ -292,7 +303,8 @@ __global__ void __launch_bounds__(kLinThreads) linear_kernel(const LinearKernelP
   }
 }
 
-// new_state = last (rf-1) samples of [old_state | in[0:n)] (slot table: into the other buffer of each stream's pair)
+// new_state = last (rf-1) samples of [old_state | in[0:n)] (slot table: into the other buffer of each stream's pair, n the
+// stream's own count; a stream with n == 0 keeps its history where it is, and the host counts no flip for it)
 __global__ void linear_update_state_kernel(const LinearKernelParams p, float* __restrict__ new_state)
 {
   const int hist = p.rf - 1;
@@ -300,15 +312,19 @@ __global__ void linear_update_state_kernel(const LinearKernelParams p, float* __
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= hist)
     return;
-  const int t = p.n_frames - hist + i; // relative frame index of new history slot i
+  int n = p.n_frames;
   const float* old_st = p.state + (size_t)stream * p.state_stride;
   float* new_st = new_state + (size_t)stream * p.state_stride;
   if (p.slots)
   {
     const StreamRef r = p.slots[stream];
+    if (r.frames == 0)
+      return;
+    n = r.frames;
     old_st = (r.alt ? p.state_alt : p.state) + (size_t)r.stream * p.state_stride;
     new_st = (r.alt ? p.state : p.state_alt) + (size_t)r.stream * p.state_stride;
   }
+  const int t = n - hist + i; // relative frame index of new history slot i
   float v;
   if (t >= 0)
     v = p.in[(size_t)stream * p.in_stride + t];
@@ -1575,7 +1591,8 @@ void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch
     if (slots)
     {
       for (int b = 0; b < batch; b++)
-        m->stream_flips[(size_t)m->h_slots[(size_t)b].stream]++; // (only the parity against lin_flips matters)
+        if (m->h_slots[(size_t)b].frames > 0) // (a stream that ran no frames stays on its side)
+          m->stream_flips[(size_t)m->h_slots[(size_t)b].stream]++; // (only the parity against lin_flips matters)
       return;
     }
     std::swap(m->d_state, m->d_state_tmp);
@@ -1662,17 +1679,20 @@ bool prefix_needs_table(const nam_b200_model* m, int batch)
   return false;
 }
 
-// The call's slot table (streams[i], or i when streams == nullptr) -> m->h_slots -> the device table, ordered on `st` before
-// the launches that read it.  The host copy is pageable: cudaMemcpyAsync stages it before returning, so the next call may
-// rebuild it at once.  The device table waits for the previous table call's launches (slots_free).
-const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t st)
+// The call's slot table (streams[i], or i when streams == nullptr; counts[i] frames, or n_frames each when counts ==
+// nullptr) -> m->h_slots -> the device table, ordered on `st` before the launches that read it.  The host copy is
+// pageable: cudaMemcpyAsync stages it before returning, so the next call may rebuild it at once.  The device table waits
+// for the previous table call's launches (slots_free).
+const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, int n_frames, const int32_t* counts,
+                              cudaStream_t st)
 {
   const bool linear = m->spec.arch == Arch::Linear;
   for (int i = 0; i < n; i++)
   {
     const int32_t s = streams ? streams[i] : i;
-    m->h_slots[(size_t)i] =
-      StreamRef{s, m->stream_clock[(size_t)s], (linear && ((m->lin_flips - m->stream_flips[(size_t)s]) & 1u)) ? 1 : 0, 0};
+    m->h_slots[(size_t)i] = StreamRef{s, m->stream_clock[(size_t)s],
+                                      (linear && ((m->lin_flips - m->stream_flips[(size_t)s]) & 1u)) ? 1 : 0,
+                                      counts ? counts[i] : n_frames};
   }
   if (m->slots_used)
     CUDA_CHECK(cudaStreamWaitEvent(st, m->slots_free, 0));
@@ -1680,14 +1700,15 @@ const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, 
   return m->d_slots;
 }
 
-// After the launches of a table call on `st`: the listed streams' histories (and the handle's clock) moved on by n_frames
+// After the launches of a table call on `st`: each listed stream's history moved on by its own count, the handle's clock
+// by the call's n_frames (the longest count)
 void finish_table_call(nam_b200_model* m, int n, int n_frames, cudaStream_t st)
 {
   CUDA_CHECK(cudaEventRecord(m->slots_free, st));
   m->slots_used = true;
   m->t_base += (uint32_t)n_frames;
   for (int i = 0; i < n; i++)
-    m->stream_clock[(size_t)m->h_slots[(size_t)i].stream] += (uint32_t)n_frames;
+    m->stream_clock[(size_t)m->h_slots[(size_t)i].stream] += (uint32_t)m->h_slots[(size_t)i].frames;
   m->streams_identical = false;
   recount_phase(m);
 }
@@ -1703,12 +1724,13 @@ void finish_contiguous_call(nam_b200_model* m, int batch, int n_frames)
 
 // Run the hot path on device buffers and advance the stream clocks.  `streams` (n = batch entries): the call's positions
 // run these streams, each from its own clock.  nullptr: streams [0, batch) -- launched without a table while all of them
-// are in phase, else with the identity table (a stream that sat out calls continues from its own clock).
+// are in phase, else with the identity table (a stream that sat out calls continues from its own clock).  `counts`
+// (with `streams`): position i runs counts[i] <= n_frames frames; n_frames stays the buffers' frame pitch.
 void run_device(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                long out_stride, cudaStream_t st, const int32_t* streams = nullptr)
+                long out_stride, cudaStream_t st, const int32_t* streams = nullptr, const int32_t* counts = nullptr)
 {
   const bool table = streams != nullptr || prefix_needs_table(m, batch);
-  const StreamRef* slots = table ? upload_slots(m, streams, batch, st) : nullptr;
+  const StreamRef* slots = table ? upload_slots(m, streams, batch, n_frames, counts, st) : nullptr;
   switch (m->spec.arch)
   {
     case Arch::WaveNet: launch_wavenet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, 0, slots); break;
@@ -2415,11 +2437,15 @@ int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i
 // streams [0, n).  Large WaveNet batches are pipelined in chunks of whole kernel waves so that the copies of chunk c+1 /
 // c-1 overlap the kernel of chunk c (the kernel is compute-bound; the copies would otherwise add ~18 %); a chunk of a table
 // call is a sub-range of the table.  Returns once `out` is filled.
+// `counts` (nam_b200_process_streams_ragged_f32, with `streams`): row i runs counts[i] <= n_frames frames, n_frames stays
+// the staging pitch.  The kernels never write past a row's count, so when some row is short the output staging is zeroed
+// first and the padding arrives as zeros.
 void process_host(nam_b200_model* m, const int32_t* streams, int n, const float* in, float* out, int n_frames, int64_t in_stride,
-                  int64_t out_stride)
+                  int64_t out_stride, const int32_t* counts = nullptr)
 {
   const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
   const size_t row = (size_t)n_frames * sizeof(float);
+  const bool padded = counts != nullptr && std::any_of(counts, counts + n, [&](int32_t c) { return c < n_frames; });
   const int chunk = wavenet_chunk_streams(m);
   if (chunk > 0 && n >= 2 * chunk && (size_t)n * row >= ((size_t)8 << 20))
   {
@@ -2437,7 +2463,7 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
     }
     const bool table = streams != nullptr || prefix_needs_table(m, n);
     CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-    const StreamRef* slots = table ? upload_slots(m, streams, n, m->stream) : nullptr;
+    const StreamRef* slots = table ? upload_slots(m, streams, n, n_frames, counts, m->stream) : nullptr;
     for (int c = 0; c < n_chunks; c++)
     {
       const int s0 = c * chunk, nb = std::min(chunk, n - s0);
@@ -2448,6 +2474,8 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
                                    (size_t)nb, cudaMemcpyHostToDevice, m->copy_in));
       CUDA_CHECK(cudaEventRecord(e_in, m->copy_in));
       CUDA_CHECK(cudaStreamWaitEvent(m->stream, e_in, 0));
+      if (padded)
+        CUDA_CHECK(cudaMemsetAsync(dout, 0, (size_t)nb * row, m->stream));
       launch_wavenet(m, din, dout, nb, n_frames, n_frames, n_frames, m->stream, s0, slots ? slots + s0 : nullptr);
       CUDA_CHECK(cudaEventRecord(e_k, m->stream));
       CUDA_CHECK(cudaStreamWaitEvent(m->copy_out, e_k, 0));
@@ -2467,8 +2495,10 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
   // (multi-channel models: a stream's row is its channel planes back to back)
   CUDA_CHECK(cudaMemcpy2DAsync(m->d_in, ci * row, in, (size_t)in_stride * sizeof(float), ci * row, (size_t)n,
                                cudaMemcpyHostToDevice, m->stream));
+  if (padded)
+    CUDA_CHECK(cudaMemsetAsync(m->d_out, 0, (size_t)n * co * row, m->stream));
   CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-  run_device(m, m->d_in, m->d_out, n, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream, streams);
+  run_device(m, m->d_in, m->d_out, n, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream, streams, counts);
   CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
   CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)out_stride * sizeof(float), m->d_out, co * row, co * row, (size_t)n,
                                cudaMemcpyDeviceToHost, m->stream));
@@ -2504,6 +2534,31 @@ int check_process_streams_args(const nam_b200_model* m, const char* fn, const in
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": out_stride " + std::to_string(out_stride)
                                                  + " < out_channels x n_frames = " + std::to_string(co * n_frames));
   return NAM_B200_OK;
+}
+
+// nam_b200_process_streams_ragged_f32(_device): the per-row counts, then the checks of a process_streams call of
+// *n_max = max(n_frames[i]) frames
+int check_ragged_args(const nam_b200_model* m, const char* fn, const int32_t* streams, int n, const int32_t* n_frames,
+                      const void* in, const void* out, int64_t in_stride, int64_t out_stride, int* n_max)
+{
+  const std::string f(fn);
+  *n_max = 0;
+  if (!m->is_reset)
+    return fail(NAM_B200_ERR_STATE, f + " called before reset");
+  if (n > 0 && n <= m->opts.max_batch)
+  {
+    if (!n_frames)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": null n_frames");
+    for (int i = 0; i < n; i++)
+    {
+      if (n_frames[i] < 0 || n_frames[i] > m->max_frames)
+        return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": n_frames[" + std::to_string(i) + "] = " + std::to_string(n_frames[i])
+                                                     + " outside [0, max_frames=" + std::to_string(m->max_frames)
+                                                     + "] of the last reset");
+      *n_max = std::max(*n_max, (int)n_frames[i]);
+    }
+  }
+  return check_process_streams_args(m, fn, streams, n, in, out, *n_max, in_stride, out_stride);
 }
 
 // host records go through device staging in groups of at most this many bytes
@@ -3206,6 +3261,41 @@ int nam_b200_process_streams_f32_device(nam_b200_model* m, const int32_t* stream
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
     CUDA_CHECK(cudaEventRecord(m->ev0, st));
     run_device(m, in_device, out_device, n, n_frames, (long)in_stride, (long)out_stride, st, streams);
+    CUDA_CHECK(cudaEventRecord(m->ev1, st));
+    m->timing_valid = true;
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_process_streams_ragged_f32(nam_b200_model* m, const int32_t* streams, int n, const int32_t* n_frames,
+                                        const float* in, float* out, int64_t in_stride, int64_t out_stride)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int n_max = 0;
+    const int rc =
+      check_ragged_args(m, "process_streams_ragged_f32", streams, n, n_frames, in, out, in_stride, out_stride, &n_max);
+    if (rc != NAM_B200_OK || n == 0 || n_max == 0)
+      return rc;
+    process_host(m, streams, n, in, out, n_max, in_stride, out_stride, n_frames);
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_process_streams_ragged_f32_device(nam_b200_model* m, const int32_t* streams, int n, const int32_t* n_frames,
+                                               const float* in_device, float* out_device, int64_t in_stride,
+                                               int64_t out_stride, void* cuda_stream)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int n_max = 0;
+    const int rc = check_ragged_args(m, "process_streams_ragged_f32_device", streams, n, n_frames, in_device, out_device,
+                                     in_stride, out_stride, &n_max);
+    if (rc != NAM_B200_OK || n == 0 || n_max == 0)
+      return rc;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
+    CUDA_CHECK(cudaEventRecord(m->ev0, st));
+    run_device(m, in_device, out_device, n, n_max, (long)in_stride, (long)out_stride, st, streams, n_frames);
     CUDA_CHECK(cudaEventRecord(m->ev1, st));
     m->timing_valid = true;
     return NAM_B200_OK;

@@ -758,10 +758,12 @@ __device__ __forceinline__ void array_forward(const WaveNetKernelParams& p, cons
 }
 
 // Lock-step mode epilogue: the stream's rings take the last `lookback` columns of the call from hist (every tile
-// copies the columns it owns).  Runs after every tile of the stream has finished reading the rings.
-template <int C, int S, int NT, int LQ>
+// copies the columns it owns).  Runs after every tile of the stream has finished reading the rings.  TBL: n is the
+// stream's own count from the slot table (without one the call's p.n_frames).
+template <int C, int S, int NT, int LQ, bool TBL>
 __device__ __forceinline__ void ls_write_back(const WaveNetKernelParams& p, const ArrayDesc& A, float* state,
-                                              const float4* hist_a, const int t0, const uint32_t tabs0, const int tv)
+                                              const float4* hist_a, const int t0, const uint32_t tabs0, const int tv,
+                                              const int n)
 {
   constexpr int P = C / 4;
   const int NC = p.hist_cols;
@@ -786,7 +788,7 @@ __device__ __forceinline__ void ls_write_back(const WaveNetKernelParams& p, cons
     for (int j = 0; j < S; j++)
     {
       const int f = (j * NT + (int)threadIdx.x) & ((1 << LQ) - 1);
-      if (f < tv && t0 + f >= p.n_frames - lookback)
+      if (f < tv && t0 + f >= (TBL ? n : p.n_frames) - lookback)
       {
 #pragma unroll
         for (int pl = 0; pl < P; pl++)
@@ -860,8 +862,26 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
       yout[j] = p.out + sc * p.out_stride;
       fj[j] = trel & (FQ - 1);
     }
+    // TBL: every position runs its own count of frames (slots[].frames <= p.n_frames).  Q == 1: the tiles stop at the
+    // stream's count -- a tile-parallel CTA whose tile starts past it has no work, and no tile of the stream waits on it.
+    // Q > 1: the slot's tiles run to its longest stream and a sub-tile past its stream's count gets Tv = 0, the masking
+    // of a slot beyond the batch.
+    int n_pos[S]; // frames of the stream of this thread's j-th frame (TBL only)
+    int t_stop = t_end;
+    if constexpr (TBL)
+    {
+#pragma unroll
+      for (int j = 0; j < S; j++)
+        n_pos[j] = live[j] ? p.slots[position(j)].frames : 0;
+      int n_max = 0;
+#pragma unroll
+      for (int q = 0; q < Q; q++)
+        if (stream0 + q < p.batch)
+          n_max = max(n_max, p.slots[stream0 + q].frames);
+      t_stop = min(t_end, n_max);
+    }
 
-    for (int t0 = t_begin; t0 < t_end; t0 += FQ)
+    for (int t0 = t_begin; t0 < t_stop; t0 += FQ)
     {
       const int tv = min(FQ, p.n_frames - t0);
       const uint32_t tabs0 = p.t_base + (uint32_t)t0;
@@ -874,7 +894,10 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
 #pragma unroll
       for (int j = 0; j < S; j++)
       {
-        Tv[j] = live[j] ? tv : 0;
+        if constexpr (TBL)
+          Tv[j] = min(FQ, max(0, n_pos[j] - t0));
+        else
+          Tv[j] = live[j] ? tv : 0;
         x[j][0] = (fj[j] < Tv[j]) ? __ldg(xin[j] + t0 + fj[j]) : 0.0f;
         cond[j] = x[j][0]; // no condition_dsp: condition == input (model.cpp:781)
       }
@@ -928,15 +951,16 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
           yout[j][t0 + fj[j]] = p.head_scale * y[j]; // model.cpp:888-897
       if constexpr (LS)
       {
-        // every tile of the stream is done with the rings -> rewrite them from hist for the next call
+        // every tile of the stream is done with the rings -> rewrite them from hist for the next call.  (TBL: only the
+        // stream's own tiles ever publish -- the tiles past its count have no work -- so the wait stops at them.)
         ls_publish_wait(ts, kLsFinalStep, 0);
-        for (int k = tid; k < p.tiles_per_stream; k += NT)
+        for (int k = tid; k < (TBL ? (n_pos[0] + FQ - 1) >> LQ : p.tiles_per_stream); k += NT)
           ls_spin_until_above(ts.mine - ts.tile_i + k, kLsFinalStep);
         __syncthreads();
         const uint32_t tabs_s = TBL ? p.slots[position(0)].clock + (uint32_t)t0 : tabs0;
-        ls_write_back<C0, S, NT, LQ>(p, p.arrays[0], state[0], hist0, t0, tabs_s, Tv[0]);
+        ls_write_back<C0, S, NT, LQ, TBL>(p, p.arrays[0], state[0], hist0, t0, tabs_s, Tv[0], n_pos[0]);
         if constexpr (C1 != 0)
-          ls_write_back<C1, S, NT, LQ>(p, p.arrays[1], state[0], hist1, t0, tabs_s, Tv[0]);
+          ls_write_back<C1, S, NT, LQ, TBL>(p, p.arrays[1], state[0], hist1, t0, tabs_s, Tv[0], n_pos[0]);
       }
     }
     __syncthreads(); // the next streams reuse the tile

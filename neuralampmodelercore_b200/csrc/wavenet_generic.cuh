@@ -324,15 +324,17 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
   const int ci = p.net.in_channels, co = p.net.out_channels;
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
-    // position s of the call: state row and clock from the slot table, or row s at the handle's clock
+    // position s of the call: state row, clock and frame count from the slot table, or row s at the handle's clock
+    // (p.n_frames stays the channel-plane pitch)
     const uint32_t clock = TBL ? p.slots[s].clock : p.t_base;
+    const int n = TBL ? p.slots[s].frames : p.n_frames;
     c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
-    for (int t0 = 0; t0 < p.n_frames; t0 += kGenTile)
+    for (int t0 = 0; t0 < n; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;
-      c.valid = f < p.n_frames;
+      c.valid = f < n;
       c.t = clock + (uint32_t)f;
       float in[kGenMaxVec], out[kGenMaxVec], cond[kGenMaxVec];
       for (int ch = 0; ch < ci; ch++)
@@ -370,13 +372,14 @@ __global__ void __launch_bounds__(kGenTile) convnet_kernel(const __grid_constant
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
     const uint32_t clock = TBL ? p.slots[s].clock : p.t_base;
+    const int n = TBL ? p.slots[s].frames : p.n_frames;
     c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
-    for (int t0 = 0; t0 < p.n_frames; t0 += kGenTile)
+    for (int t0 = 0; t0 < n; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;
-      c.valid = f < p.n_frames;
+      c.valid = f < n;
       c.t = clock + (uint32_t)f;
       float x[kGenMaxVec], z[kGenMaxVec];
       for (int ch = 0; ch < N.in_channels; ch++)

@@ -45,7 +45,9 @@ struct GParams
   long in_stride, out_stride;
   int batch, n_frames;
   unsigned t_base;
-  const StreamRef* slots; // nullptr: position s is state row s at t_base; else row slots[s].stream at slots[s].clock
+  // nullptr: position s is state row s at t_base running n_frames frames; else row slots[s].stream at slots[s].clock
+  // running slots[s].frames
+  const StreamRef* slots;
 };
 
 constexpr int kTile = 128; // frames per tile == threads per CTA (the ring geometry of generic_pack.cpp assumes it)
@@ -327,13 +329,14 @@ extern "C" __global__ void __launch_bounds__(namb200_gspec::kTile) wavenet_gener
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
     const unsigned clock = p.slots ? p.slots[s].clock : p.t_base;
+    const int n = p.slots ? p.slots[s].frames : p.n_frames; // (p.n_frames stays the channel-plane pitch)
     c.st = p.state + (size_t)(p.slots ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
-    for (int t0 = 0; t0 < p.n_frames; t0 += kTile)
+    for (int t0 = 0; t0 < n; t0 += kTile)
     {
       const int f = t0 + (int)threadIdx.x;
-      c.valid = f < p.n_frames;
+      c.valid = f < n;
       c.t = clock + (unsigned)f;
       float in[kGenMaxVec], out[kGenMaxVec], cond[kGenMaxVec];
 #pragma unroll

@@ -397,7 +397,7 @@ __device__ __forceinline__ void wavenet_lat_body(const LatParams& p)
   c.bars = bars;
   c.state = p.state + (size_t)(p.slots ? p.slots[stream].stream : stream) * p.state_stride;
   c.tabs0 = p.slots ? p.slots[stream].clock : p.t_base;
-  c.n = p.n_frames;
+  c.n = p.slots ? p.slots[stream].frames : p.n_frames; // (one stream per CTA: its own count)
   c.f = tid & (F - 1);
   const int g = tid / F; // warp-uniform: F is a multiple of 32
   if (tid < spec::NL)

@@ -416,7 +416,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   c.bars = bars;
   c.state = state;
   c.tabs0 = clock;
-  c.n = p.n_frames;
+  c.n = TBL ? p.slots[stream].frames : p.n_frames; // (one stream per CTA: its own count)
   c.f = tid & (F - 1);
   c.g = tid / F;
   const float xv = (c.f < c.n) ? p.in[(size_t)stream * p.in_stride + c.f] : 0.0f;

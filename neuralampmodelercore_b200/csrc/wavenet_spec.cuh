@@ -59,7 +59,8 @@ struct SlotRef
 {
   int stream; // state row of this position of the call
   u32 clock; // where that row's history ends
-  int alt, pad;
+  int alt;
+  int frames; // frames this position runs, <= n_frames (the buffers' frame pitch)
 };
 
 struct SpecParams
@@ -73,8 +74,9 @@ struct SpecParams
   u32 t_base; // absolute frame index of in[:, 0] (mod 2^32)
   float* scratch; // S = 2: [grid][scratch_stride] floats, a CTA's stream pair in the interleaved layout
   long scratch_stride; // 2 * state_stride
-  // slot table (nullptr: position b is state row b at t_base): position b uses row slots[b].stream at slots[b].clock; inputs
-  // and outputs stay indexed by position.  The stream-pair variant (S = 2) is never given one.
+  // slot table (nullptr: position b is state row b at t_base, running n_frames frames): position b uses row slots[b].stream
+  // at slots[b].clock and runs slots[b].frames frames; inputs and outputs stay indexed by position.  The stream-pair
+  // variant (S = 2) is never given one.
   const SlotRef* slots;
 };
 
@@ -709,6 +711,7 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
     float* const state_a = p.state + (size_t)(table ? p.slots[sa].stream : sa) * p.state_stride;
     float* const state_b = p.state + (size_t)sb * p.state_stride;
     const u32 clock_a = table ? p.slots[sa].clock : p.t_base;
+    const int n_a = table ? p.slots[sa].frames : p.n_frames; // the stream's own frames (CTA-uniform: one stream)
     const float* xin_a = p.in + (size_t)sa * p.in_stride;
     const float* xin_b = p.in + (size_t)sb * p.in_stride;
     float* yout_a = p.out + (size_t)sa * p.out_stride;
@@ -722,9 +725,9 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
       fence_async_all(); // my scratch stores (generic proxy) -> the bulk loads below
       __syncthreads();
     }
-    for (int t0 = 0; t0 < p.n_frames; t0 += T)
+    for (int t0 = 0; t0 < n_a; t0 += T)
     {
-      c.tv = min(T, p.n_frames - t0);
+      c.tv = min(T, n_a - t0);
       c.tabs0 = clock_a + (u32)t0;
       request_layer_history<0, NT, S>(c, IntC<spec::A[0].layer0>{});
       V x[1];
@@ -1038,7 +1041,8 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
     const int sc = min(stream, p.batch - 1);
     float* state = p.state + (size_t)(p.slots ? p.slots[sc].stream : sc) * p.state_stride;
     const u32 clock = p.slots ? p.slots[sc].clock : p.t_base; // per q: the streams of a CTA need not share a clock
-    const float xv = (live && f < p.n_frames) ? __ldg(p.in + (size_t)sc * p.in_stride + f) : 0.0f;
+    const int n = !live ? 0 : p.slots ? p.slots[sc].frames : p.n_frames; // ... nor a frame count
+    const float xv = (f < n) ? __ldg(p.in + (size_t)sc * p.in_stride + f) : 0.0f;
     const float x[1] = {xv};
     constexpr int C0 = spec::A[0].C;
     float head0[C0], hout0[C0], ho0[spec::A[0].HOUT];
@@ -1046,7 +1050,7 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
     for (int o = 0; o < C0; o++)
       head0[o] = 0.0f;
     float y;
-    array_forward_short<0, spec::NA - 1, NT, FQ>(spec_smem, state, pol, clock, p.n_frames, f, live, x, xv, head0, hout0, ho0);
+    array_forward_short<0, spec::NA - 1, NT, FQ>(spec_smem, state, pol, clock, n, f, live, x, xv, head0, hout0, ho0);
     if constexpr (spec::NA == 1)
       y = ho0[0];
     else
@@ -1058,10 +1062,10 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
       for (int o = 0; o < C1; o++)
         head1[o] = ho0[o];
       __syncthreads(); // (the last layer's tap reads are fenced by its B1; this orders the rechannel's tile stores too)
-      array_forward_short<AI1, -1, NT, FQ>(spec_smem, state, pol, clock, p.n_frames, f, live, hout0, xv, head1, hout1, ho1);
+      array_forward_short<AI1, -1, NT, FQ>(spec_smem, state, pol, clock, n, f, live, hout0, xv, head1, hout1, ho1);
       y = ho1[0];
     }
-    if (live && f < p.n_frames)
+    if (f < n)
       p.out[(size_t)sc * p.out_stride + f] = spec::head_scale * y;
     __syncthreads(); // the next slot rewrites the tile
   }

@@ -317,10 +317,14 @@ class DSP:
         if rc != 0:
             _raise(rc, self._lib)
 
-    def process_streams(self, streams, x: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
+    def process_streams(self, streams, x: np.ndarray, out: Optional[np.ndarray] = None, n_frames=None) -> np.ndarray:
         """Run only the listed streams (distinct, any order): row i of x belongs to streams[i], and each stream continues
         from its own history, however many calls it sat out; unlisted streams are untouched.  x: (n, frames) float32, or
-        (n, in_channels, frames) for a multi-channel model -> out of the same layout with out_channels."""
+        (n, in_channels, frames) for a multi-channel model -> out of the same layout with out_channels.
+
+        n_frames (a sequence, one count per row): a ragged call -- row i runs only its first n_frames[i] frames, frames is
+        max(n_frames), the rest of the row is padding that is never read and comes back as zeros; each stream advances
+        by its own count (0: the stream is left exactly as it was)."""
         s = self._streams(streams)
         x = np.asarray(x)
         if x.ndim == 3:
@@ -343,21 +347,49 @@ class DSP:
         elif (not isinstance(out, np.ndarray) or out.dtype != np.float32 or out.shape != shape
               or not out.flags["C_CONTIGUOUS"]):
             raise ValueError(f"out must be a C-contiguous float32 array of shape {shape}")
-        self._check(self._lib.nam_b200_process_streams_f32(self._h, self._i32p(s), len(s), x.ctypes.data_as(C.c_void_p),
-                                                           out.ctypes.data_as(C.c_void_p), n, self.in_channels * n,
-                                                           self.out_channels * n))
+        if n_frames is None:
+            self._check(self._lib.nam_b200_process_streams_f32(self._h, self._i32p(s), len(s), x.ctypes.data_as(C.c_void_p),
+                                                               out.ctypes.data_as(C.c_void_p), n, self.in_channels * n,
+                                                               self.out_channels * n))
+            return out
+        counts = self._counts(n_frames, len(s))
+        if len(counts) and int(counts.max()) != n:
+            raise ValueError(f"x has {n} frames per row; a ragged call takes max(n_frames) = {int(counts.max())}")
+        self._check(self._lib.nam_b200_process_streams_ragged_f32(
+            self._h, self._i32p(s), len(s), self._i32p(counts), x.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p),
+            self.in_channels * n, self.out_channels * n))
         return out
 
-    def process_streams_device(self, streams, in_ptr: int, out_ptr: int, n_frames: int, in_stride: int | None = None,
+    def process_streams_device(self, streams, in_ptr: int, out_ptr: int, n_frames, in_stride: int | None = None,
                                out_stride: int | None = None, cuda_stream: int = 0) -> None:
         """process_streams on device buffers (e.g. torch.Tensor.data_ptr()), asynchronous on `cuda_stream` (0 = the
-        handle's stream).  Strides in floats between rows, default channels x n_frames."""
+        handle's stream).  Strides in floats between rows, default channels x n_frames.  n_frames: an int, or a sequence
+        of one count per row for a ragged call (rows laid out at a pitch of max(n_frames), padding neither read nor
+        written)."""
         s = self._streams(streams)
-        self._check(self._lib.nam_b200_process_streams_f32_device(
-            self._h, self._i32p(s), len(s), C.c_void_p(in_ptr), C.c_void_p(out_ptr), int(n_frames),
-            int(in_stride if in_stride is not None else self.in_channels * n_frames),
-            int(out_stride if out_stride is not None else self.out_channels * n_frames),
-            C.c_void_p(cuda_stream) if cuda_stream else None))
+        st = C.c_void_p(cuda_stream) if cuda_stream else None
+        if isinstance(n_frames, (int, np.integer)):
+            self._check(self._lib.nam_b200_process_streams_f32_device(
+                self._h, self._i32p(s), len(s), C.c_void_p(in_ptr), C.c_void_p(out_ptr), int(n_frames),
+                int(in_stride if in_stride is not None else self.in_channels * n_frames),
+                int(out_stride if out_stride is not None else self.out_channels * n_frames), st))
+            return
+        counts = self._counts(n_frames, len(s))
+        n_max = int(counts.max()) if len(counts) else 0
+        self._check(self._lib.nam_b200_process_streams_ragged_f32_device(
+            self._h, self._i32p(s), len(s), self._i32p(counts), C.c_void_p(in_ptr), C.c_void_p(out_ptr),
+            int(in_stride if in_stride is not None else self.in_channels * n_max),
+            int(out_stride if out_stride is not None else self.out_channels * n_max), st))
+
+    @staticmethod
+    def _counts(n_frames, n: int) -> np.ndarray:
+        """Per-row frame counts of a ragged call -> int32 array (range checks are the library's)."""
+        counts = np.ascontiguousarray(np.asarray(n_frames, dtype=np.int64).reshape(-1))
+        if len(counts) != n:
+            raise ValueError(f"n_frames has {len(counts)} entries for {n} streams")
+        if len(counts) and (counts.min() < np.iinfo(np.int32).min or counts.max() > np.iinfo(np.int32).max):
+            raise ValueError("n_frames entries must fit in int32")
+        return counts.astype(np.int32)
 
     # ---- per-stream state (include/nam_b200.h: records, per-stream clocks) ------------------------------------------
     @property
