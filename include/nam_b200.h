@@ -166,6 +166,52 @@ int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, in
  * describes its default (largest) sub-model.  Returns 0, or the error codes of create. */
 int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t capacity);
 
+/* ---- model banks: one handle, streams of different captures of one architecture ----------------------------------------
+ * A bank is a handle created from K >= 1 .nam documents of one shape; each of its max_batch streams is bound to one of the
+ * K models, and every process call runs each listed stream with its own model's weights, in the launches an ordinary
+ * handle's call of that batch takes.  Which documents can share a bank:
+ *   - every one served by the fused WaveNet kernel family (wavenet.nam, a1_standard, A2-Lite and A2-Full shapes): not the
+ *     general kernel (gated, FiLM, ...), ConvNet, LSTM, Linear, SlimmableContainer files or slimmable WaveNets;
+ *   - models 1.. equal to model 0 in everything but their weights: layer arrays, channels, kernel sizes, dilations,
+ *     activations and their parameters, hence the packed kernel layout and blob length; the config object apart from its
+ *     unused head_scale field (head_scale is the last weight, so it is per model); the expected sample rate.
+ *   Refusals (NAM_B200_ERR_UNSUPPORTED for a model outside the family, NAM_B200_ERR_MODEL for a mismatch) name the first
+ *   offending model index and the field.  jit = 1 is refused (a model-specialised kernel compiles one model's weights into
+ *   its code); jit = 0 or 3 silently keeps the precompiled kernels, and nam_b200_jit_note says so.  kernel_geometry 4 (the
+ *   general kernel) is refused.  A bank of one document is exactly nam_b200_create_from_json / _from_file, JIT included.
+ * All streams start bound to model 0.  Every call of this header works on a bank:
+ *   - process calls (nam_b200_process_f32 and _device, process_streams*, the ragged calls, the planar DSP::process on stream
+ *     0, the pipelined host path): each stream runs its own model;
+ *   - nam_b200_reset / nam_b200_prewarm: every stream ends in the (prewarmed) state of its own model;
+ *   - reset_streams: as nam_b200_assign_streams to each stream's current model;
+ *   - copy_streams: the destination takes the source's model along with its state;
+ *   - export_streams: a record carries the fingerprint of its stream's model;
+ *   - import_streams: accepts a record of any model of the bank and binds the stream to it (with duplicate documents the
+ *     lowest such index); a fingerprint outside the bank is refused, naming it.  A session therefore moves between a bank
+ *     and an ordinary handle of its model in either direction.
+ * Device memory: the K blobs (a1_standard: ~14k floats each) and K output scales, plus K "model rows" of per-stream state
+ * (a1_standard: 196 KB each) that hold every model's freshly reset state: reset prewarms them together and copies each
+ * stream its model's row; reset_streams and assign_streams copy them again (one launch whatever the mix). */
+int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const nam_b200_options* opts, nam_b200_model** out);
+int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out);
+/* K of a bank; 1 for every other handle (so model index 0 is valid on every handle). */
+int nam_b200_bank_size(const nam_b200_model* m);
+/* Bind streams[i] to model models[i] and put it in the state of a freshly reset handle of that model (the reset_streams
+ * contract, per model); every other stream is untouched.  Checked on the host like the other stream lists (distinct
+ * streams in [0, max_batch), model indices in [0, bank_size), after reset); a refusal names the entry.  On an ordinary
+ * handle, models all 0 is nam_b200_reset_streams. */
+int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, const int32_t* models);
+/* out[i] = the model streams[i] is bound to. */
+int nam_b200_stream_models(const nam_b200_model* m, const int32_t* streams, int n, int32_t* out);
+/* nam_b200_get_info with model k's document-level fields (loudness, input / output levels, expected sample rate, weight
+ * count): what a server needs per capture for normalisation.  k = 0 on an ordinary handle is nam_b200_get_info. */
+int nam_b200_bank_model_info(const nam_b200_model* m, int k, nam_b200_info* info);
+/* Host-only, no CUDA: can these documents share a bank?  A JSON object: ok, n_models, reason (the first offending model
+ * index and field; "" when ok), fingerprints (each parsed model's record fingerprint, an unsigned
+ * 64-bit integer as in nam_b200_state_layout_json).  Returns 0 whatever
+ * the verdict; NAM_B200_ERR_INVALID_ARGUMENT when the buffer is too small. */
+int nam_b200_bank_check_json(const char* const* texts, int n_models, char* out, int64_t capacity);
+
 /* Batched throughput entry: `batch` (<= max_batch) streams, stream b reads
  * in[b*in_stride .. +n_frames) and writes out[b*out_stride .. +n_frames); n_frames <= max_frames.
  * Multi-channel models (in_channels / out_channels of nam_b200_info != 1; WaveNet: NAM/wavenet/model.cpp:809-820,

@@ -7,12 +7,14 @@ nam::DSP / nam::get_dsp interface (dsp.py) used by tests and bench.py.
 from ._build import build, LIB_PATH  # noqa: F401
 from .dsp import (  # noqa: F401
     DSP,
+    bank_check,
     CudaUnavailableError,
     NamFileValidationError,
     UnsupportedModelError,
     disable_fast_tanh,
     enable_fast_tanh,
     get_dsp,
+    get_dsp_bank,
     inspect,
     jit_prepare,
     measure_fp32_tflops,
@@ -27,6 +29,8 @@ __all__ = [
     "LIB_PATH",
     "DSP",
     "get_dsp",
+    "get_dsp_bank",
+    "bank_check",
     "inspect",
     "jit_prepare",
     "submodels",

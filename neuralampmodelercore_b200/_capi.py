@@ -105,6 +105,13 @@ EXPORTED_SYMBOLS = [
     "nam_b200_process_streams_f32_device",
     "nam_b200_process_streams_ragged_f32",
     "nam_b200_process_streams_ragged_f32_device",
+    "nam_b200_create_bank_from_json",
+    "nam_b200_create_bank_from_files",
+    "nam_b200_bank_size",
+    "nam_b200_assign_streams",
+    "nam_b200_stream_models",
+    "nam_b200_bank_model_info",
+    "nam_b200_bank_check_json",
 ]
 
 
@@ -193,6 +200,17 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_process_streams_f32_device.argtypes = [vp, i32p, C.c_int, vp, vp, C.c_int, C.c_int64, C.c_int64, vp]
     lib.nam_b200_process_streams_ragged_f32.argtypes = [vp, i32p, C.c_int, i32p, vp, vp, C.c_int64, C.c_int64]
     lib.nam_b200_process_streams_ragged_f32_device.argtypes = [vp, i32p, C.c_int, i32p, vp, vp, C.c_int64, C.c_int64, vp]
+    strv = C.POINTER(C.c_char_p)
+    lib.nam_b200_create_bank_from_json.argtypes = [strv, C.c_int, C.POINTER(Options), C.POINTER(vp)]
+    lib.nam_b200_create_bank_from_files.argtypes = [strv, C.c_int, C.POINTER(Options), C.POINTER(vp)]
+    lib.nam_b200_bank_size.argtypes = [vp]
+    lib.nam_b200_assign_streams.argtypes = [vp, i32p, C.c_int, i32p]
+    lib.nam_b200_stream_models.argtypes = [vp, i32p, C.c_int, i32p]
+    lib.nam_b200_bank_model_info.argtypes = [vp, C.c_int, C.POINTER(Info)]
+    lib.nam_b200_bank_check_json.argtypes = [strv, C.c_int, C.c_char_p, C.c_int64]
+    for name in ("nam_b200_create_bank_from_json", "nam_b200_create_bank_from_files", "nam_b200_bank_size",
+                 "nam_b200_assign_streams", "nam_b200_stream_models", "nam_b200_bank_model_info", "nam_b200_bank_check_json"):
+        getattr(lib, name).restype = C.c_int
     for name in ("nam_b200_reset_streams", "nam_b200_copy_streams", "nam_b200_export_streams", "nam_b200_import_streams",
                  "nam_b200_export_streams_device", "nam_b200_import_streams_device", "nam_b200_state_layout_json",
                  "nam_b200_process_streams_f32", "nam_b200_process_streams_f32_device",

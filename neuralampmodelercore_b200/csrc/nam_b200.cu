@@ -474,6 +474,19 @@ struct nam_b200_model
   bool slots_used = false;
   int n_out_of_phase = 0; // streams whose history does not end at t_base (Linear: or sits in the other buffer)
   size_t refs_capacity = 0;
+  // model bank (nam_b200_create_bank_*): bank_size >= 2 WaveNets of one WaveNetPlan, each stream bound to one of them.
+  // d_weights holds their blobs weight_stride floats apart, d_head_scales their output scales, d_bank_headers their record
+  // headers.  State rows max_batch .. max_batch + bank_size - 1 are the models' fresh rows: reset prewarms them together
+  // and copies them out; reset_streams / assign_streams copy them again.  Their histories end at fresh_clock.
+  // Ordinary handles: bank_size 1, stream_model all 0, no extra rows.
+  int bank_size = 1;
+  std::vector<ModelSpec> bank_specs; // model k's document (bank_size entries; bank_specs[0] is `spec`'s twin)
+  std::vector<StateRecordHeader> bank_headers;
+  std::vector<int32_t> stream_model;
+  long weight_stride = 0;
+  float* d_head_scales = nullptr;
+  uint32_t* d_bank_headers = nullptr;
+  uint32_t fresh_clock = 0;
   unsigned char* d_xfer = nullptr; // staging of host records, scratch rows of copies and LSTM prewarms
   size_t xfer_bytes = 0;
   // staging
@@ -530,6 +543,10 @@ struct nam_b200_model
       cudaEventDestroy(slots_free);
     if (d_xfer)
       cudaFree(d_xfer);
+    if (d_head_scales)
+      cudaFree(d_head_scales);
+    if (d_bank_headers)
+      cudaFree(d_bank_headers);
     if (d_in)
       cudaFree(d_in);
     if (d_out)
@@ -1223,6 +1240,8 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   kp.n_frames = n_frames;
   kp.t_base = m->t_base;
   kp.head_scale = plan.head_scale;
+  kp.weight_stride = m->weight_stride;
+  kp.head_scales = m->d_head_scales; // (a bank's calls always carry a table: prefix_needs_table)
   kp.n_arrays = plan.n_arrays;
   for (size_t i = 0; i < plan.arrays.size(); i++)
     kp.arrays[i] = plan.arrays[i];
@@ -1667,10 +1686,13 @@ void recount_phase(nam_b200_model* m)
     n += in_phase(m, s) ? 0 : 1;
   m->n_out_of_phase = n;
 }
-// Must a contiguous call over streams [0, batch) carry an identity slot table (one of them sat out calls)?  O(1) while every
-// stream is in phase (a handle that always runs all its streams).
+// Must a contiguous call over streams [0, batch) carry an identity slot table (one of them sat out calls, or the handle is a
+// model bank, whose table carries each position's model)?  O(1) while every stream is in phase (a handle that always runs
+// all its streams).
 bool prefix_needs_table(const nam_b200_model* m, int batch)
 {
+  if (m->bank_size > 1)
+    return true;
   if (m->n_out_of_phase == 0)
     return false;
   for (int b = 0; b < batch; b++)
@@ -1683,6 +1705,13 @@ bool prefix_needs_table(const nam_b200_model* m, int batch)
 // nullptr) -> m->h_slots -> the device table, ordered on `st` before the launches that read it.  The host copy is
 // pageable: cudaMemcpyAsync stages it before returning, so the next call may rebuild it at once.  The device table waits
 // for the previous table call's launches (slots_free).
+const StreamRef* push_slots(nam_b200_model* m, int n, cudaStream_t st)
+{
+  if (m->slots_used)
+    CUDA_CHECK(cudaStreamWaitEvent(st, m->slots_free, 0));
+  CUDA_CHECK(cudaMemcpyAsync(m->d_slots, m->h_slots.data(), (size_t)n * sizeof(StreamRef), cudaMemcpyHostToDevice, st));
+  return m->d_slots;
+}
 const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, int n_frames, const int32_t* counts,
                               cudaStream_t st)
 {
@@ -1690,14 +1719,12 @@ const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, 
   for (int i = 0; i < n; i++)
   {
     const int32_t s = streams ? streams[i] : i;
+    // (Linear: the buffer the history is in; every other architecture: the stream's model, 0 outside a bank)
     m->h_slots[(size_t)i] = StreamRef{s, m->stream_clock[(size_t)s],
-                                      (linear && ((m->lin_flips - m->stream_flips[(size_t)s]) & 1u)) ? 1 : 0,
+                                      linear ? ((m->lin_flips - m->stream_flips[(size_t)s]) & 1u ? 1 : 0) : m->stream_model[(size_t)s],
                                       counts ? counts[i] : n_frames};
   }
-  if (m->slots_used)
-    CUDA_CHECK(cudaStreamWaitEvent(st, m->slots_free, 0));
-  CUDA_CHECK(cudaMemcpyAsync(m->d_slots, m->h_slots.data(), (size_t)n * sizeof(StreamRef), cudaMemcpyHostToDevice, st));
-  return m->d_slots;
+  return push_slots(m, n, st);
 }
 
 // After the launches of a table call on `st`: each listed stream's history moved on by its own count, the handle's clock
@@ -1786,9 +1813,16 @@ void ensure_pinned(nam_b200_model* m, size_t floats)
 }
 
 // Zero the state, set the trained initial state where the architecture has one.
+// state rows of the handle: one per stream, plus a bank's model rows
+int state_rows(const nam_b200_model* m)
+{
+  return m->opts.max_batch + (m->bank_size > 1 ? m->bank_size : 0);
+}
+
 void init_state(nam_b200_model* m)
 {
-  const size_t total = (size_t)m->state_stride * m->opts.max_batch;
+  const size_t total = (size_t)m->state_stride * state_rows(m);
+  m->fresh_clock = 0;
   CUDA_CHECK(cudaMemsetAsync(m->d_state, 0, total * sizeof(float), m->stream));
   if (m->spec.arch == Arch::LSTM)
   {
@@ -1837,9 +1871,11 @@ void prewarm(nam_b200_model* m)
   // DSP::prewarm continues from the instance's CURRENT state (dsp.cpp:67-101).  Straight after init_state every stream
   // would compute the same thing: stream 0 runs, its state is broadcast.  Once the streams have seen different audio
   // (a standalone nam_b200_prewarm, or a Reset of an LSTM, which keeps its running state) all of them are prewarmed.
-  const int nb = m->streams_identical ? 1 : m->opts.max_batch;
+  // (a bank's streams run different models: nam_b200_reset prewarms it through prewarm_bank, a standalone prewarm runs
+  // every stream with its own model)
+  const bool identical = m->streams_identical && m->bank_size == 1;
+  const int nb = identical ? 1 : m->opts.max_batch;
   CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)nb * bs * ci * sizeof(float), m->stream));
-  const bool identical = m->streams_identical;
   int done = 0;
   while (done < ps)
   {
@@ -1931,7 +1967,8 @@ void export_records(nam_b200_model* m, const int32_t* streams, int n, unsigned c
   for (int i = 0; i < n; i++)
   {
     const size_t s = (size_t)streams[i];
-    refs[(size_t)i] = StreamRef{streams[i], m->stream_clock[s], (linear && ((m->lin_flips - m->stream_flips[s]) & 1u)) ? 1 : 0, 0};
+    refs[(size_t)i] = StreamRef{streams[i], m->stream_clock[s],
+                                linear ? ((m->lin_flips - m->stream_flips[s]) & 1u ? 1 : 0) : m->stream_model[s], 0};
   }
   StatePackParams p{};
   p.segs = m->d_state_descs;
@@ -1944,6 +1981,7 @@ void export_records(nam_b200_model* m, const int32_t* streams, int n, unsigned c
   p.rec = dst;
   p.rec_stride = stride;
   std::memcpy(p.header, &m->record_header, sizeof p.header);
+  p.headers = m->d_bank_headers; // (a bank: the header of each stream's model)
   state_pack_kernel<<<state_grid(m, n), kStateThreads, 0, st>>>(p);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
@@ -2032,6 +2070,54 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
   }
   copy_rows(m, m->d_state, d_refs, rows, nullptr, n, m->stream);
   mark_written(m, streams, n);
+}
+
+// ---- model banks: fresh state per model --------------------------------------------------------------------------------
+// The listed streams take the fresh row of the model they are bound to (one row-copy launch whatever the mix); their
+// histories then end at fresh_clock.  A bank's calls carry every stream's clock, so the streams need not be in step.
+void bank_fan_out(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t st)
+{
+  std::vector<StreamRef> refs((size_t)2 * n);
+  for (int i = 0; i < n; i++)
+  {
+    refs[(size_t)i] = StreamRef{m->opts.max_batch + m->stream_model[(size_t)streams[i]], 0, 0, 0};
+    refs[(size_t)(n + i)] = StreamRef{streams[i], 0, 0, 0};
+  }
+  const StreamRef* d_refs = upload_refs(m, refs, st);
+  copy_rows(m, m->d_state, d_refs + n, m->d_state, d_refs, n, st);
+  for (int i = 0; i < n; i++)
+    m->stream_clock[(size_t)streams[i]] = m->fresh_clock;
+  m->streams_identical = false;
+  recount_phase(m);
+}
+
+// DSP::prewarm for a bank straight after init_state: the bank_size model rows are prewarmed together -- position k of each
+// launch is model k's row, running model k -- exactly like prewarm() runs stream 0 of an ordinary handle, then every stream
+// takes its model's row.
+void prewarm_bank(nam_b200_model* m)
+{
+  const int ps = m->spec.prewarm_samples, K = m->bank_size;
+  const int bs = std::max(m->max_frames, 1);
+  if (ps > 0)
+  {
+    ensure_staging(m, (size_t)std::max(m->opts.max_batch, K) * bs);
+    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)K * bs * sizeof(float), m->stream));
+    for (int done = 0; done < ps; done += bs)
+    {
+      for (int k = 0; k < K; k++)
+        m->h_slots[(size_t)k] = StreamRef{m->opts.max_batch + k, m->t_base, k, bs};
+      launch_wavenet(m, m->d_in, m->d_out, K, bs, bs, bs, m->stream, 0, push_slots(m, K, m->stream));
+      CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
+      m->slots_used = true;
+      m->t_base += (uint32_t)bs;
+    }
+  }
+  m->fresh_clock = m->t_base;
+  std::vector<int32_t> all((size_t)m->opts.max_batch);
+  for (int s = 0; s < m->opts.max_batch; s++)
+    all[(size_t)s] = s;
+  bank_fan_out(m, all.data(), m->opts.max_batch, m->stream);
+  CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 
 int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_model** out)
@@ -2216,6 +2302,7 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
       CUDA_CHECK(cudaMalloc(&m->d_state_tmp, std::max<size_t>(state_total, 4) * sizeof(float)));
     m->stream_clock.assign((size_t)m->opts.max_batch, 0u);
     m->stream_flips.assign((size_t)m->opts.max_batch, 0u);
+    m->stream_model.assign((size_t)m->opts.max_batch, 0);
     m->h_slots.assign((size_t)m->opts.max_batch, StreamRef{0, 0u, 0, 0});
     CUDA_CHECK(cudaMalloc(&m->d_slots, (size_t)m->opts.max_batch * sizeof(StreamRef)));
     CUDA_CHECK(cudaEventCreateWithFlags(&m->slots_free, cudaEventDisableTiming));
@@ -2406,9 +2493,12 @@ int check_records(const nam_b200_model* m, const void* buf, int n, int64_t strid
   return NAM_B200_OK;
 }
 
-// the header of record i (for stream `stream`) must be this model's
-int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i, int stream)
+// the header of record i (for stream `stream`) must be this model's -- a bank's: one of its models', *model receives the
+// lowest such index (0 on an ordinary handle)
+int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i, int stream, int* model = nullptr)
 {
+  if (model)
+    *model = 0;
   StateRecordHeader h;
   std::memcpy(&h, rec, sizeof h);
   const StateRecordHeader& want = m->record_header;
@@ -2427,6 +2517,18 @@ int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i
   if (h.payload_floats != want.payload_floats)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "payload float count " + std::to_string(h.payload_floats)
                                                  + ", the model's record holds " + std::to_string(want.payload_floats));
+  if (m->bank_size > 1)
+  {
+    for (int k = 0; k < m->bank_size; k++)
+      if (h.fingerprint == m->bank_headers[(size_t)k].fingerprint)
+      {
+        if (model)
+          *model = k;
+        return NAM_B200_OK;
+      }
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "model fingerprint " + hex[0] + " is none of the "
+                                                 + std::to_string(m->bank_size) + " models of this bank");
+  }
   if (h.fingerprint != want.fingerprint)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "model fingerprint " + hex[0] + " is not this model's (" + hex[1]
                                                  + "): a record of another model, or of another slimmable size");
@@ -2563,6 +2665,200 @@ int check_ragged_args(const nam_b200_model* m, const char* fn, const int32_t* st
 
 // host records go through device staging in groups of at most this many bytes
 constexpr size_t kRecordStagingBytes = (size_t)64 << 20;
+
+// ---- model banks: which documents can share one handle ---------------------------------------------------------------
+// Every model must be served by the fused WaveNet kernel, and models 1.. must match model 0 in everything but their weights
+// (head_scale, the last weight, included): the same WaveNetPlan apart from the blob's values, the same config object, the
+// same expected sample rate (as ContainerModel requires of its sub-models).
+struct BankCheck
+{
+  int code = NAM_B200_OK;
+  std::string reason; // names the first offending model and the field
+  std::vector<WaveNetPlan> plans;
+};
+
+// "" when model k (spec s, plan p) matches model 0 (s0, p0), else the first difference
+std::string bank_difference(int k, const ModelSpec& s, const WaveNetPlan& p, const ModelSpec& s0, const WaveNetPlan& p0)
+{
+  const std::string mk = "model " + std::to_string(k) + " differs from model 0 in ";
+  auto num = [](double v) { return json::number_to_string(v); };
+  auto differ = [&](const std::string& field, double a, double b) { return mk + field + " (" + num(a) + " vs " + num(b) + ")"; };
+  if (!(s.sample_rate == s0.sample_rate))
+    return differ("expected sample_rate", s.sample_rate, s0.sample_rate);
+  const WaveNetSpec &w = s.wavenet, &w0 = s0.wavenet;
+  if (w.arrays.size() != w0.arrays.size())
+    return differ("the number of layer arrays", (double)w.arrays.size(), (double)w0.arrays.size());
+  for (size_t a = 0; a < w.arrays.size(); a++)
+  {
+    const ArraySpec &A = w.arrays[a], &A0 = w0.arrays[a];
+    const std::string at = "array " + std::to_string(a) + " ";
+    const struct
+    {
+      const char* name;
+      int v, v0;
+    } fields[] = {{"input_size", A.input_size, A0.input_size},
+                  {"condition_size", A.condition_size, A0.condition_size},
+                  {"channels", A.channels, A0.channels},
+                  {"bottleneck", A.bottleneck, A0.bottleneck},
+                  {"head_size", A.head_size, A0.head_size},
+                  {"head kernel_size", A.head_kernel, A0.head_kernel},
+                  {"head dilation", A.head_dilation, A0.head_dilation},
+                  {"head_bias", A.head_bias ? 1 : 0, A0.head_bias ? 1 : 0},
+                  {"number of layers (dilations)", (int)A.layers.size(), (int)A0.layers.size()}};
+    for (const auto& f : fields)
+      if (f.v != f.v0)
+        return differ(at + f.name, f.v, f.v0);
+    for (size_t l = 0; l < A.layers.size(); l++)
+    {
+      const LayerSpec &L = A.layers[l], &L0 = A0.layers[l];
+      const std::string lt = at + "layer " + std::to_string(l) + " ";
+      if (L.conv.kernel != L0.conv.kernel)
+        return differ(lt + "kernel_size", L.conv.kernel, L0.conv.kernel);
+      if (L.conv.dilation != L0.conv.dilation)
+        return differ(lt + "dilation", L.conv.dilation, L0.conv.dilation);
+      if (L.gating != L0.gating)
+        return differ(lt + "gating", (int)L.gating, (int)L0.gating);
+      if (L.act.type != L0.act.type)
+        return differ(lt + "activation", (int)L.act.type, (int)L0.act.type);
+      if (L.act.slope != L0.act.slope || L.act.slopes != L0.act.slopes || L.act.min_val != L0.act.min_val
+          || L.act.max_val != L0.act.max_val || L.act.min_slope != L0.act.min_slope || L.act.max_slope != L0.act.max_slope)
+        return mk + lt + "activation parameters";
+    }
+  }
+  // the packed form (padded channels, ring layout, descriptors, blob length) -- equal whenever the above is, kept as the
+  // statement of what the kernels rely on
+  bool same = p.n_arrays == p0.n_arrays && p.blob.size() == p0.blob.size() && p.state_floats == p0.state_floats
+              && std::equal(p.cp, p.cp + kMaxArrays, p0.cp) && std::equal(p.creal, p.creal + kMaxArrays, p0.creal)
+              && p.arrays.size() == p0.arrays.size() && p.layers.size() == p0.layers.size();
+  same = same && std::memcmp(p.arrays.data(), p0.arrays.data(), p.arrays.size() * sizeof(ArrayDesc)) == 0
+         && std::memcmp(p.layers.data(), p0.layers.data(), p.layers.size() * sizeof(LayerDesc)) == 0;
+  if (!same)
+    return mk + "the packed kernel layout (descriptors, rings or blob length)";
+  if (s.config_fingerprint != s0.config_fingerprint)
+    return mk + "its config object (apart from the weights and head_scale)";
+  return "";
+}
+
+BankCheck check_bank(const std::vector<ModelSpec>& specs)
+{
+  BankCheck r;
+  auto refuse = [&](int code, const std::string& why) {
+    r.code = code;
+    r.reason = why;
+    return r;
+  };
+  if (specs.empty())
+    return refuse(NAM_B200_ERR_INVALID_ARGUMENT, "n_models must be >= 1");
+  for (size_t k = 0; k < specs.size(); k++)
+  {
+    const ModelSpec& s = specs[k];
+    const std::string mk = "model " + std::to_string(k) + ": ";
+    if (s.arch == Arch::Container)
+      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture: a slimmable document (SlimmableContainer or slimmable "
+                                                   "WaveNet); a bank serves plain WaveNets of the fused kernel family");
+    if (s.arch != Arch::WaveNet)
+      return refuse(NAM_B200_ERR_UNSUPPORTED,
+                    mk + "architecture " + s.architecture + ": a bank serves WaveNets of the fused kernel family only");
+    WaveNetPlan plan = plan_wavenet(s);
+    if (plan.eligible && !(s.in_channels == 1 && s.out_channels == 1))
+    {
+      plan.eligible = false;
+      plan.why_not = "multi-channel in / out";
+    }
+    if (plan.eligible && wavenet_smem_bytes(plan, 1) > 227 * 1024)
+    {
+      plan.eligible = false;
+      plan.why_not = "packed weights + tile exceed the shared memory of the fused kernel";
+    }
+    if (!plan.eligible)
+      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "kernel: not served by the fused WaveNet kernel (" + plan.why_not
+                                                + "); a bank serves the fused family only (the general kernel does not take banks)");
+    r.plans.push_back(std::move(plan));
+  }
+  for (size_t k = 1; k < specs.size(); k++)
+  {
+    const std::string d = bank_difference((int)k, specs[k], r.plans[k], specs[0], r.plans[0]);
+    if (!d.empty())
+      return refuse(NAM_B200_ERR_MODEL, d);
+  }
+  return r;
+}
+
+// A bank handle: an ordinary handle of model 0 on the precompiled kernels, then the blobs, output scales, record headers
+// and model rows of all K models
+void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const std::vector<WaveNetPlan>& plans)
+{
+  const int K = (int)specs.size();
+  m->bank_size = K;
+  m->weight_stride = (long)((m->plan.blob.size() + 3) & ~(size_t)3); // (float4 loads of every blob)
+  std::vector<float> blobs((size_t)K * m->weight_stride, 0.0f), scales((size_t)K);
+  for (int k = 0; k < K; k++)
+  {
+    std::copy(plans[(size_t)k].blob.begin(), plans[(size_t)k].blob.end(), blobs.begin() + (size_t)k * m->weight_stride);
+    scales[(size_t)k] = plans[(size_t)k].head_scale;
+  }
+  CUDA_CHECK(cudaFree(m->d_weights));
+  m->d_weights = nullptr;
+  CUDA_CHECK(cudaMalloc(&m->d_weights, blobs.size() * sizeof(float)));
+  CUDA_CHECK(cudaMemcpy(m->d_weights, blobs.data(), blobs.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)K * sizeof(float)));
+  CUDA_CHECK(cudaMemcpy(m->d_head_scales, scales.data(), (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
+  // the model rows behind the streams' rows
+  CUDA_CHECK(cudaFree(m->d_state));
+  m->d_state = nullptr;
+  CUDA_CHECK(cudaMalloc(&m->d_state, (size_t)m->state_stride * state_rows(m) * sizeof(float)));
+  // slot tables of up to max(max_batch, K) positions (prewarm_bank runs the K model rows in one launch)
+  const size_t n_slots = (size_t)std::max(m->opts.max_batch, K);
+  m->h_slots.assign(n_slots, StreamRef{0, 0u, 0, 0});
+  CUDA_CHECK(cudaFree(m->d_slots));
+  m->d_slots = nullptr;
+  CUDA_CHECK(cudaMalloc(&m->d_slots, n_slots * sizeof(StreamRef)));
+  if (m->state_error.empty())
+  {
+    for (int k = 0; k < K; k++)
+      m->bank_headers.push_back(state_record_header(specs[(size_t)k], m->record_floats));
+    CUDA_CHECK(cudaMalloc(&m->d_bank_headers, (size_t)K * kStateHeaderBytes));
+    CUDA_CHECK(cudaMemcpy(m->d_bank_headers, m->bank_headers.data(), (size_t)K * kStateHeaderBytes, cudaMemcpyHostToDevice));
+  }
+  m->bank_specs = std::move(specs);
+  m->spec_state = 0;
+  m->spec_note = "model bank of " + std::to_string(K) + " models: the precompiled kernels, which read each stream's weights as "
+                 "data (a model-specialised kernel compiles one model's weights into its code)";
+  init_state(m);
+  CUDA_CHECK(cudaStreamSynchronize(m->stream));
+}
+
+int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opts, nam_b200_model** out)
+{
+  const BankCheck bc = check_bank(specs);
+  if (bc.code != NAM_B200_OK)
+    return fail(bc.code, "model bank: " + bc.reason);
+  nam_b200_options o;
+  nam_b200_default_options(&o);
+  if (user_opts)
+  {
+    std::memcpy(&o, user_opts, std::min<size_t>(sizeof o, (size_t)std::max(user_opts->struct_size, 0)));
+    o.struct_size = sizeof o;
+  }
+  if (o.jit == 1)
+    return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: jit = 1 (required) cannot be met: a model-specialised kernel compiles "
+                                          "one model's weights into its code, a bank's streams each bring their own");
+  if (o.kernel_geometry == 4)
+    return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: kernel_geometry 4 (the general kernel) does not take banks");
+  o.jit = 2; // jit 0 / 3: the precompiled kernels, silently (nam_b200_jit_note says why)
+  nam_b200_model* h = nullptr;
+  const int rc = create_common(ModelSpec(specs[0]), &o, &h);
+  if (rc != NAM_B200_OK)
+    return rc;
+  std::unique_ptr<nam_b200_model> m(h);
+  const int rc2 = guarded(m.get(), [&]() -> int {
+    setup_bank(m.get(), std::move(specs), bc.plans);
+    return NAM_B200_OK;
+  });
+  if (rc2 == NAM_B200_OK)
+    *out = m.release();
+  return rc2;
+}
 
 } // namespace
 
@@ -2894,28 +3190,26 @@ int64_t nam_b200_submodel_json(const char* nam_json_text, int index, double* max
   }
 }
 
-int nam_b200_get_info(const nam_b200_model* m, nam_b200_info* info)
+// the handle's info with the document-level fields (loudness, levels, sample rate, weights) of `spec`
+static int fill_info(const nam_b200_model* m, const ModelSpec& spec, nam_b200_info* info)
 {
-  m = active_model(m);
-  if (!m || !info)
-    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
   nam_b200_info r;
   std::memset(&r, 0, sizeof(r));
   r.struct_size = sizeof(nam_b200_info);
-  r.architecture = (int)m->spec.arch;
-  r.in_channels = m->spec.in_channels;
-  r.out_channels = m->spec.out_channels;
-  r.prewarm_samples = m->spec.prewarm_samples;
+  r.architecture = (int)spec.arch;
+  r.in_channels = spec.in_channels;
+  r.out_channels = spec.out_channels;
+  r.prewarm_samples = spec.prewarm_samples;
   r.max_batch = m->opts.max_batch;
   r.max_frames = m->max_frames;
-  r.has_loudness = m->spec.loudness.has_value();
-  r.has_input_level = m->spec.input_level.has_value();
-  r.has_output_level = m->spec.output_level.has_value();
-  r.expected_sample_rate = m->spec.sample_rate;
-  r.loudness = m->spec.loudness.value_or(0.0);
-  r.input_level_dbu = m->spec.input_level.value_or(0.0);
-  r.output_level_dbu = m->spec.output_level.value_or(0.0);
-  r.n_weights = (int64_t)m->spec.n_weights;
+  r.has_loudness = spec.loudness.has_value();
+  r.has_input_level = spec.input_level.has_value();
+  r.has_output_level = spec.output_level.has_value();
+  r.expected_sample_rate = spec.sample_rate;
+  r.loudness = spec.loudness.value_or(0.0);
+  r.input_level_dbu = spec.input_level.value_or(0.0);
+  r.output_level_dbu = spec.output_level.value_or(0.0);
+  r.n_weights = (int64_t)spec.n_weights;
   r.state_bytes_per_stream = (int64_t)m->state_stride * 4;
   r.flops_per_frame = m->flops_per_frame;
   r.kernel_variant = m->variant;
@@ -2926,6 +3220,14 @@ int nam_b200_get_info(const nam_b200_model* m, nam_b200_info* info)
   std::memcpy(info, &r, n);
   info->struct_size = user_size;
   return NAM_B200_OK;
+}
+
+int nam_b200_get_info(const nam_b200_model* m, nam_b200_info* info)
+{
+  m = active_model(m);
+  if (!m || !info)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
+  return fill_info(m, m->spec, info);
 }
 
 int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
@@ -2967,11 +3269,11 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
     m->is_reset = true;
     CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
     if (m->opts.prewarm_on_reset)
-      prewarm(m);
+      (m->bank_size > 1 ? prewarm_bank : prewarm)(m);
     CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
     // every stream is now in the state of a freshly reset one: keep stream 0's record for nam_b200_reset_streams (an LSTM
-    // keeps its running state across a Reset, so its streams are re-derived per call instead)
-    if (m->spec.arch != Arch::LSTM && m->state_error.empty())
+    // keeps its running state across a Reset, so its streams are re-derived per call instead; a bank keeps model rows)
+    if (m->spec.arch != Arch::LSTM && m->state_error.empty() && m->bank_size == 1)
     {
       const int32_t s0 = 0;
       export_records(m, &s0, 1, m->d_fresh, 0, m->stream);
@@ -3015,6 +3317,8 @@ int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int
       return rc;
     if (m->spec.arch == Arch::LSTM)
       lstm_reset_rows(m, streams, n, fresh != 0);
+    else if (m->bank_size > 1)
+      bank_fan_out(m, streams, n, m->stream); // each stream's own model's fresh row
     else
       import_records(m, streams, n, m->d_fresh, 0, m->stream); // (fresh or not: Reset forgets the past)
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -3053,15 +3357,18 @@ int nam_b200_copy_streams(nam_b200_model* m, const int32_t* src, const int32_t* 
       copy_rows(m, m->d_state_tmp, d_refs + n, scratch + rows, nullptr, n, m->stream);
     }
     std::vector<uint32_t> clock((size_t)n), flips((size_t)n);
+    std::vector<int32_t> model((size_t)n); // (a bank: the destination takes the source's model along with its state)
     for (int i = 0; i < n; i++)
     {
       clock[(size_t)i] = m->stream_clock[(size_t)src[i]];
       flips[(size_t)i] = m->stream_flips[(size_t)src[i]];
+      model[(size_t)i] = m->stream_model[(size_t)src[i]];
     }
     for (int i = 0; i < n; i++)
     {
       m->stream_clock[(size_t)dst[i]] = clock[(size_t)i];
       m->stream_flips[(size_t)dst[i]] = flips[(size_t)i];
+      m->stream_model[(size_t)dst[i]] = model[(size_t)i];
     }
     m->streams_identical = false;
     recount_phase(m);
@@ -3105,10 +3412,13 @@ int nam_b200_import_streams(nam_b200_model* m, const int32_t* streams, int n, co
       rc = check_stream_list(m, streams, n, "streams", true);
     if (rc == NAM_B200_OK)
       rc = check_records(m, src, n, record_stride, false);
+    std::vector<int> model((size_t)std::max(n, 0));
     for (int i = 0; i < n && rc == NAM_B200_OK; i++)
-      rc = check_record_header(m, static_cast<const unsigned char*>(src) + (size_t)i * record_stride, i, streams[i]);
+      rc = check_record_header(m, static_cast<const unsigned char*>(src) + (size_t)i * record_stride, i, streams[i], &model[(size_t)i]);
     if (rc != NAM_B200_OK || n == 0)
       return rc;
+    for (int i = 0; i < n; i++) // (a bank: the stream runs the record's model from now on)
+      m->stream_model[(size_t)streams[i]] = model[(size_t)i];
     const size_t rb = record_bytes(m);
     const int group = (int)std::max<size_t>(1, kRecordStagingBytes / rb);
     ensure_xfer(m, (size_t)std::min(n, group) * rb);
@@ -3160,12 +3470,15 @@ int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, in
     CUDA_CHECK(cudaMemcpy2DAsync(headers.data(), kStateHeaderBytes, src_device, (size_t)record_stride, kStateHeaderBytes, (size_t)n,
                                  cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
+    std::vector<int> model((size_t)n);
     for (int i = 0; i < n; i++)
     {
-      rc = check_record_header(m, headers.data() + (size_t)i * kStateHeaderBytes, i, streams[i]);
+      rc = check_record_header(m, headers.data() + (size_t)i * kStateHeaderBytes, i, streams[i], &model[(size_t)i]);
       if (rc != NAM_B200_OK)
         return rc;
     }
+    for (int i = 0; i < n; i++)
+      m->stream_model[(size_t)streams[i]] = model[(size_t)i];
     import_records(m, streams, n, static_cast<const unsigned char*>(src_device), (long)record_stride, st);
     return NAM_B200_OK;
   });
@@ -3196,6 +3509,176 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
   {
     return fail(NAM_B200_ERR_MODEL, ex.what());
   }
+}
+
+// ---- model banks ---------------------------------------------------------------------------------------------------------
+int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const nam_b200_options* opts, nam_b200_model** out)
+{
+  if (!out)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
+  *out = nullptr;
+  if (n_models < 1)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: n_models = " + std::to_string(n_models) + " must be >= 1");
+  if (!texts)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: null document list");
+  if (n_models == 1)
+    return nam_b200_create_from_json(texts[0], opts, out);
+  LoadOptions lo;
+  lo.fast_tanh = opts ? (opts->fast_tanh != 0) : false;
+  std::vector<ModelSpec> specs;
+  for (int k = 0; k < n_models; k++)
+  {
+    const std::string mk = "model bank: model " + std::to_string(k) + ": ";
+    if (!texts[k])
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, mk + "null document");
+    try
+    {
+      specs.push_back(model_spec_from_text(texts[k], lo));
+    }
+    catch (const json::ParseError& ex)
+    {
+      return fail(NAM_B200_ERR_FILE, mk + ex.what());
+    }
+    catch (const std::exception& ex)
+    {
+      return fail(NAM_B200_ERR_MODEL, mk + ex.what());
+    }
+  }
+  return create_bank(std::move(specs), opts, out);
+}
+
+int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out)
+{
+  if (!out)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
+  *out = nullptr;
+  if (n_models < 1)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: n_models = " + std::to_string(n_models) + " must be >= 1");
+  if (!paths)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: null path list");
+  if (n_models == 1)
+    return nam_b200_create_from_file(paths[0], opts, out);
+  LoadOptions lo;
+  lo.fast_tanh = opts ? (opts->fast_tanh != 0) : false;
+  std::vector<ModelSpec> specs;
+  for (int k = 0; k < n_models; k++)
+  {
+    const std::string mk = "model bank: model " + std::to_string(k) + ": ";
+    if (!paths[k])
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, mk + "null path");
+    try
+    {
+      specs.push_back(model_spec_from_file(paths[k], lo));
+    }
+    catch (const NamFileValidationError& ex)
+    {
+      return fail(NAM_B200_ERR_FILE, mk + ex.what());
+    }
+    catch (const std::exception& ex)
+    {
+      return fail(NAM_B200_ERR_MODEL, mk + ex.what());
+    }
+  }
+  return create_bank(std::move(specs), opts, out);
+}
+
+int nam_b200_bank_check_json(const char* const* texts, int n_models, char* out, int64_t capacity)
+{
+  if (!out || capacity <= 0)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument or empty output buffer");
+  std::string reason;
+  std::vector<ModelSpec> specs;
+  if (n_models < 1)
+    reason = "n_models = " + std::to_string(n_models) + " must be >= 1";
+  else if (!texts)
+    reason = "null document list";
+  for (int k = 0; reason.empty() && k < n_models; k++)
+  {
+    try
+    {
+      if (!texts[k])
+        throw std::runtime_error("null document");
+      specs.push_back(model_spec_from_text(texts[k], LoadOptions{}));
+    }
+    catch (const std::exception& ex)
+    {
+      reason = "model " + std::to_string(k) + ": " + ex.what();
+    }
+  }
+  if (reason.empty())
+    reason = check_bank(specs).reason;
+  for (auto& ch : reason)
+    if (ch == '"' || ch == '\\' || ch == '\n')
+      ch = ' ';
+  std::string s = std::string("{\"ok\": ") + (reason.empty() ? "true" : "false") + ", \"n_models\": " + std::to_string(n_models)
+                  + ", \"reason\": \"" + reason + "\", \"fingerprints\": [";
+  for (size_t k = 0; k < specs.size(); k++) // (as nam_b200_state_layout_json writes them)
+    s += std::string(k ? ", " : "") + std::to_string((unsigned long long)specs[k].fingerprint);
+  s += "]}";
+  if ((int64_t)s.size() >= capacity)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "the bank check needs " + std::to_string(s.size() + 1) + " bytes, the buffer has "
+                                                 + std::to_string(capacity));
+  std::memcpy(out, s.c_str(), s.size() + 1);
+  return NAM_B200_OK;
+}
+
+int nam_b200_bank_size(const nam_b200_model* m)
+{
+  m = active_model(m);
+  if (!m)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null model handle");
+  return m->bank_size;
+}
+
+int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, const int32_t* models)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    int rc = check_state_calls(m, "assign_streams");
+    if (rc == NAM_B200_OK)
+      rc = check_stream_list(m, streams, n, "assign_streams: streams", true);
+    if (rc == NAM_B200_OK && n > 0 && !models)
+      rc = fail(NAM_B200_ERR_INVALID_ARGUMENT, "assign_streams: null model list");
+    for (int i = 0; i < n && rc == NAM_B200_OK; i++)
+      if (models[i] < 0 || models[i] >= m->bank_size)
+        rc = fail(NAM_B200_ERR_INVALID_ARGUMENT, "assign_streams: models[" + std::to_string(i) + "] = " + std::to_string(models[i])
+                                                   + ": model index outside [0, bank_size=" + std::to_string(m->bank_size) + ")");
+    if (rc != NAM_B200_OK || n == 0)
+      return rc;
+    if (m->bank_size == 1)
+      return nam_b200_reset_streams(m, streams, n, 0);
+    for (int i = 0; i < n; i++)
+      m->stream_model[(size_t)streams[i]] = models[i];
+    bank_fan_out(m, streams, n, m->stream);
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_stream_models(const nam_b200_model* m, const int32_t* streams, int n, int32_t* out)
+{
+  m = active_model(m);
+  if (!m)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null model handle");
+  const int rc = check_stream_list(m, streams, n, "stream_models: streams", false);
+  if (rc != NAM_B200_OK)
+    return rc;
+  if (n > 0 && !out)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "stream_models: null output");
+  for (int i = 0; i < n; i++)
+    out[i] = m->stream_model[(size_t)streams[i]];
+  return NAM_B200_OK;
+}
+
+int nam_b200_bank_model_info(const nam_b200_model* m, int k, nam_b200_info* info)
+{
+  m = active_model(m);
+  if (!m || !info)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
+  if (k < 0 || k >= m->bank_size)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT,
+                "bank_model_info: model index " + std::to_string(k) + " outside [0, bank_size=" + std::to_string(m->bank_size) + ")");
+  return fill_info(m, m->bank_size > 1 ? m->bank_specs[(size_t)k] : m->spec, info);
 }
 
 int nam_b200_process_f32_device(nam_b200_model* m, const float* in_device, float* out_device, int batch, int n_frames,

@@ -1029,6 +1029,31 @@ uint64_t model_fingerprint(const std::string& architecture, const json::Value& c
   return f.h;
 }
 
+// the same over the architecture and the "config" object alone, without its "head_scale" field (the reference reads the
+// scale from the last weight, model.cpp:670): equal for documents that differ in their weights only
+uint64_t config_fingerprint(const std::string& architecture, const json::Value& config)
+{
+  Fnv64 f;
+  f.str(architecture);
+  if (!config.is_object())
+  {
+    f.value(config);
+    return f.h;
+  }
+  std::vector<const std::pair<std::string, json::Value>*> members;
+  for (const auto& kv : config.members())
+    if (kv.first != "head_scale")
+      members.push_back(&kv);
+  std::sort(members.begin(), members.end(), [](auto* a, auto* b) { return a->first < b->first; });
+  f.u64(members.size());
+  for (auto* kv : members)
+  {
+    f.str(kv->first);
+    f.value(kv->second);
+  }
+  return f.h;
+}
+
 ModelSpec build_spec(const json::Value& root, const LoadOptions& opts)
 {
   if (!root.is_object())
@@ -1069,6 +1094,7 @@ ModelSpec build_spec(const json::Value& root, const LoadOptions& opts)
   }
   const json::Value& config = root.at("config");
   ms.fingerprint = model_fingerprint(ms.architecture, config, weights);
+  ms.config_fingerprint = config_fingerprint(ms.architecture, config);
   if (ms.architecture == "WaveNet" && config_is_slimmable_wavenet(config))
     build_slimmable_wavenet(ms, root, config, weights, opts);
   else if (ms.architecture == "WaveNet")

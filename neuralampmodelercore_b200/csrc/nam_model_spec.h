@@ -214,6 +214,9 @@ struct ModelSpec
   // float32 bits of the weights: the identity of a model's state layout and arithmetic, independent of load options
   // (fast_tanh) and of how the document was spelled.  Stamped into per-stream state records (stream_state.h).
   uint64_t fingerprint = 0;
+  // the same hash without the weights and the config's unused "head_scale" field: equal for documents that differ only in
+  // their weights (model banks, nam_b200_create_bank_from_json)
+  uint64_t config_fingerprint = 0;
   WaveNetSpec wavenet;
   LstmSpec lstm;
   LinearSpec linear;

@@ -29,6 +29,7 @@ struct StatePackParams
   unsigned char* rec; // record i at rec + i * rec_stride
   long rec_stride;
   uint32_t header[kStateHeaderBytes / 4];
+  const uint32_t* headers; // model bank: record s takes headers[refs[s].model] (kStateHeaderBytes each); nullptr: header
 };
 
 __global__ void __launch_bounds__(kStateThreads) state_pack_kernel(const __grid_constant__ StatePackParams p)
@@ -41,7 +42,8 @@ __global__ void __launch_bounds__(kStateThreads) state_pack_kernel(const __grid_
     const StreamRef r = p.refs[s];
     unsigned char* rec = p.rec + (size_t)s * p.rec_stride;
     if (blockIdx.x == 0 && threadIdx.x < kStateHeaderBytes / 4)
-      reinterpret_cast<uint32_t*>(rec)[threadIdx.x] = p.header[threadIdx.x];
+      reinterpret_cast<uint32_t*>(rec)[threadIdx.x] =
+        p.headers ? p.headers[(size_t)r.model * (kStateHeaderBytes / 4) + threadIdx.x] : p.header[threadIdx.x];
     if (i >= d.items)
       continue;
     const float* __restrict__ st = (r.alt ? p.state_alt : p.state) + (size_t)r.stream * p.state_stride + d.dev_off;

@@ -90,6 +90,10 @@ struct WaveNetKernelParams
   // slot table (nullptr: position b of the call is state row b, its history ending at t_base): position b uses state row
   // slots[b].stream, whose history ends at slots[b].clock.  Inputs, outputs, hist and tile flags stay indexed by position.
   const StreamRef* slots;
+  // model bank (table calls only): position b runs model slots[b].model, whose blob is at weights + model * weight_stride
+  // and whose output scale is head_scales[model].  head_scales == nullptr: one model (weights, head_scale).
+  long weight_stride;
+  const float* head_scales;
 };
 
 } // namespace namb200

@@ -813,13 +813,16 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
   float4* tile = smem4 + (p.n_weight_floats + 3) / 4;
 
   const int tid = threadIdx.x;
-  // weights -> shared memory, once per CTA
+  // weights -> shared memory, once per CTA.  TBL: once per model the CTA meets (a bank's positions run their own models):
+  // the blob is reloaded only when the next pass's model is not the one in shared memory.
+  if constexpr (!TBL)
   {
     const float4* src = reinterpret_cast<const float4*>(p.weights);
     for (int i = tid; i < (p.n_weight_floats + 3) / 4; i += NT)
       smem4[i] = __ldg(src + i);
+    __syncthreads();
   }
-  __syncthreads();
+  int loaded = -1; // TBL: the model whose blob is in shared memory
 
   // classic mode: persistent CTA, slots of Q streams, all tiles of a call in turn.  Tile-parallel mode (Q == 1):
   // this CTA owns ONE (stream, tile) and hands its ring columns to the next tile's CTA layer by layer.
@@ -866,103 +869,138 @@ __global__ void __launch_bounds__(NT, MINB) wavenet_fused_kernel(const __grid_co
     // stream's count -- a tile-parallel CTA whose tile starts past it has no work, and no tile of the stream waits on it.
     // Q > 1: the slot's tiles run to its longest stream and a sub-tile past its stream's count gets Tv = 0, the masking
     // of a slot beyond the batch.
-    int n_pos[S]; // frames of the stream of this thread's j-th frame (TBL only)
-    int t_stop = t_end;
+    // TBL, model banks: the slot runs one pass per distinct model among its positions (Q == 1: one pass).  A pass masks the
+    // sub-tiles of the other models with Tv = 0 -- their state stays bit for bit -- so a homogeneous slot costs one pass.
+    int n_all[S]; // frames of the stream of this thread's j-th frame (TBL only)
+    unsigned todo = 0; // TBL: sub-tiles of the slot still to run
     if constexpr (TBL)
     {
 #pragma unroll
       for (int j = 0; j < S; j++)
-        n_pos[j] = live[j] ? p.slots[position(j)].frames : 0;
-      int n_max = 0;
+        n_all[j] = live[j] ? p.slots[position(j)].frames : 0;
 #pragma unroll
       for (int q = 0; q < Q; q++)
         if (stream0 + q < p.batch)
-          n_max = max(n_max, p.slots[stream0 + q].frames);
-      t_stop = min(t_end, n_max);
+          todo |= 1u << q;
     }
-
-    for (int t0 = t_begin; t0 < t_stop; t0 += FQ)
+    do
     {
-      const int tv = min(FQ, p.n_frames - t0);
-      const uint32_t tabs0 = p.t_base + (uint32_t)t0;
-      // LS: this stream's history buffer at the first plane of each array
-      float4* const hist_s = LS ? reinterpret_cast<float4*>(p.hist + (size_t)stream0 * p.hist_stride) : nullptr;
-      float4* const hist0 = LS ? hist_s + (size_t)p.hist_plane0[0] * p.hist_cols : nullptr;
-      float4* const hist1 = LS ? hist_s + (size_t)p.hist_plane0[1] * p.hist_cols : nullptr;
-      int Tv[S];
-      float x[S][1], cond[S];
+      int n_pos[S]; // TBL: n_all within this pass, 0 outside it
+      int t_stop = t_end;
+      float head_scale = p.head_scale;
+      if constexpr (TBL)
+      {
+        const int mdl = p.slots[stream0 + __ffs(todo) - 1].model;
+        unsigned pass = 0;
+        int n_max = 0;
 #pragma unroll
-      for (int j = 0; j < S; j++)
-      {
-        if constexpr (TBL)
-          Tv[j] = min(FQ, max(0, n_pos[j] - t0));
-        else
-          Tv[j] = live[j] ? tv : 0;
-        x[j][0] = (fj[j] < Tv[j]) ? __ldg(xin[j] + t0 + fj[j]) : 0.0f;
-        cond[j] = x[j][0]; // no condition_dsp: condition == input (model.cpp:781)
-      }
-      float y[S];
-      if constexpr (C1 == 0)
-      {
-        u64 head0[S][C0 / 2];
+        for (int q = 0; q < Q; q++)
+          if (((todo >> q) & 1u) && p.slots[stream0 + q].model == mdl)
+          {
+            pass |= 1u << q;
+            n_max = max(n_max, p.slots[stream0 + q].frames);
+          }
+        todo &= ~pass;
 #pragma unroll
         for (int j = 0; j < S; j++)
-#pragma unroll
-          for (int q = 0; q < C0 / 2; q++)
-            head0[j][q] = 0ull; // model.cpp:469
-        float hout0[S][C0], ho0[S][1];
-        array_forward<1, C0, 1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
-                                               head0, hout0, ho0);
+          n_pos[j] = ((pass >> ((Q == 1 ? 0 : j * NT + tid) >> LQ)) & 1u) ? n_all[j] : 0;
+        t_stop = min(t_end, n_max);
+        if (mdl != loaded && t_begin < t_stop) // (uniform: every thread reads the same table entries)
+        {
+          __syncthreads(); // the previous pass is done with the blob and the tile
+          const float4* src = reinterpret_cast<const float4*>(p.weights + (size_t)mdl * p.weight_stride);
+          for (int i = tid; i < (p.n_weight_floats + 3) / 4; i += NT)
+            smem4[i] = __ldg(src + i);
+          __syncthreads();
+          loaded = mdl;
+        }
+        if (p.head_scales != nullptr)
+          head_scale = p.head_scales[mdl];
+      }
+
+      for (int t0 = t_begin; t0 < t_stop; t0 += FQ)
+      {
+        const int tv = min(FQ, p.n_frames - t0);
+        const uint32_t tabs0 = p.t_base + (uint32_t)t0;
+        // LS: this stream's history buffer at the first plane of each array
+        float4* const hist_s = LS ? reinterpret_cast<float4*>(p.hist + (size_t)stream0 * p.hist_stride) : nullptr;
+        float4* const hist0 = LS ? hist_s + (size_t)p.hist_plane0[0] * p.hist_cols : nullptr;
+        float4* const hist1 = LS ? hist_s + (size_t)p.hist_plane0[1] * p.hist_cols : nullptr;
+        int Tv[S];
+        float x[S][1], cond[S];
 #pragma unroll
         for (int j = 0; j < S; j++)
-          y[j] = ho0[j][0];
-      }
-      else
-      {
-        float hout0[S][C0], ho0[S][C1];
+        {
+          if constexpr (TBL)
+            Tv[j] = min(FQ, max(0, n_pos[j] - t0));
+          else
+            Tv[j] = live[j] ? tv : 0;
+          x[j][0] = (fj[j] < Tv[j]) ? __ldg(xin[j] + t0 + fj[j]) : 0.0f;
+          cond[j] = x[j][0]; // no condition_dsp: condition == input (model.cpp:781)
+        }
+        float y[S];
+        if constexpr (C1 == 0)
         {
           u64 head0[S][C0 / 2];
 #pragma unroll
           for (int j = 0; j < S; j++)
 #pragma unroll
             for (int q = 0; q < C0 / 2; q++)
-              head0[j][q] = 0ull;
-          array_forward<1, C0, C1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
-                                                  head0, hout0, ho0);
+              head0[j][q] = 0ull; // model.cpp:469
+          float hout0[S][C0], ho0[S][1];
+          array_forward<1, C0, 1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
+                                                 head0, hout0, ho0);
+#pragma unroll
+          for (int j = 0; j < S; j++)
+            y[j] = ho0[j][0];
         }
-        // second array: layer input = previous array's layer output, head accumulator starts from
-        // the previous array's head output (model.cpp:846-848, :473-486)
-        u64 head1[S][C1 / 2];
+        else
+        {
+          float hout0[S][C0], ho0[S][C1];
+          {
+            u64 head0[S][C0 / 2];
+#pragma unroll
+            for (int j = 0; j < S; j++)
+#pragma unroll
+              for (int q = 0; q < C0 / 2; q++)
+                head0[j][q] = 0ull;
+            array_forward<1, C0, C1, S, NT, LQ, LS, TBL>(p, p.arrays[0], sw, tile, state, stream0, tabs0, ts, 0, hist0, t0, Tv, x, cond,
+                                                    head0, hout0, ho0);
+          }
+          // second array: layer input = previous array's layer output, head accumulator starts from
+          // the previous array's head output (model.cpp:846-848, :473-486)
+          u64 head1[S][C1 / 2];
+#pragma unroll
+          for (int j = 0; j < S; j++)
+#pragma unroll
+            for (int q = 0; q < C1 / 2; q++)
+              head1[j][q] = pack2(ho0[j][2 * q], ho0[j][2 * q + 1]);
+          float hout1[S][C1], ho1[S][1];
+          array_forward<C0, C1, 1, S, NT, LQ, LS, TBL>(p, p.arrays[1], sw, tile, state, stream0, tabs0, ts, step1, hist1, t0, Tv, hout0,
+                                                  cond, head1, hout1, ho1);
+#pragma unroll
+          for (int j = 0; j < S; j++)
+            y[j] = ho1[j][0];
+        }
 #pragma unroll
         for (int j = 0; j < S; j++)
-#pragma unroll
-          for (int q = 0; q < C1 / 2; q++)
-            head1[j][q] = pack2(ho0[j][2 * q], ho0[j][2 * q + 1]);
-        float hout1[S][C1], ho1[S][1];
-        array_forward<C0, C1, 1, S, NT, LQ, LS, TBL>(p, p.arrays[1], sw, tile, state, stream0, tabs0, ts, step1, hist1, t0, Tv, hout0,
-                                                cond, head1, hout1, ho1);
-#pragma unroll
-        for (int j = 0; j < S; j++)
-          y[j] = ho1[j][0];
+          if (fj[j] < Tv[j])
+            yout[j][t0 + fj[j]] = head_scale * y[j]; // model.cpp:888-897
+        if constexpr (LS)
+        {
+          // every tile of the stream is done with the rings -> rewrite them from hist for the next call.  (TBL: only the
+          // stream's own tiles ever publish -- the tiles past its count have no work -- so the wait stops at them.)
+          ls_publish_wait(ts, kLsFinalStep, 0);
+          for (int k = tid; k < (TBL ? (n_pos[0] + FQ - 1) >> LQ : p.tiles_per_stream); k += NT)
+            ls_spin_until_above(ts.mine - ts.tile_i + k, kLsFinalStep);
+          __syncthreads();
+          const uint32_t tabs_s = TBL ? p.slots[position(0)].clock + (uint32_t)t0 : tabs0;
+          ls_write_back<C0, S, NT, LQ, TBL>(p, p.arrays[0], state[0], hist0, t0, tabs_s, Tv[0], n_pos[0]);
+          if constexpr (C1 != 0)
+            ls_write_back<C1, S, NT, LQ, TBL>(p, p.arrays[1], state[0], hist1, t0, tabs_s, Tv[0], n_pos[0]);
+        }
       }
-#pragma unroll
-      for (int j = 0; j < S; j++)
-        if (fj[j] < Tv[j])
-          yout[j][t0 + fj[j]] = p.head_scale * y[j]; // model.cpp:888-897
-      if constexpr (LS)
-      {
-        // every tile of the stream is done with the rings -> rewrite them from hist for the next call.  (TBL: only the
-        // stream's own tiles ever publish -- the tiles past its count have no work -- so the wait stops at them.)
-        ls_publish_wait(ts, kLsFinalStep, 0);
-        for (int k = tid; k < (TBL ? (n_pos[0] + FQ - 1) >> LQ : p.tiles_per_stream); k += NT)
-          ls_spin_until_above(ts.mine - ts.tile_i + k, kLsFinalStep);
-        __syncthreads();
-        const uint32_t tabs_s = TBL ? p.slots[position(0)].clock + (uint32_t)t0 : tabs0;
-        ls_write_back<C0, S, NT, LQ, TBL>(p, p.arrays[0], state[0], hist0, t0, tabs_s, Tv[0], n_pos[0]);
-        if constexpr (C1 != 0)
-          ls_write_back<C1, S, NT, LQ, TBL>(p, p.arrays[1], state[0], hist1, t0, tabs_s, Tv[0], n_pos[0]);
-      }
-    }
+    } while (TBL && todo != 0);
     __syncthreads(); // the next streams reuse the tile
   }
 }

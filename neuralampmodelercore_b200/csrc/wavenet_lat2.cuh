@@ -321,6 +321,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   const int stream = blockIdx.x; // position in the call (input / output row)
   float* const state = p.state + (size_t)(TBL ? p.slots[stream].stream : stream) * p.state_stride;
   const uint32_t clock = TBL ? p.slots[stream].clock : p.t_base; // where this stream's history ends
+  const int model = TBL ? p.slots[stream].model : 0; // a bank's stream brings its own model's blob and output scale
 
   // window table: float4 offset of each layer's first window (prefix sums, thread li computes entry li) -- it lives
   // behind the windows; total window size is bounded by the host (lat2_smem_bytes)
@@ -369,7 +370,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
   if (tid == 0)
   {
     lat_mbar_expect_tx(bars + kMaxLayers, (uint32_t)wf4 * 16u);
-    lat_bulk_g2s(lat2_smem, p.weights, (uint32_t)wf4 * 16u, bars + kMaxLayers);
+    lat_bulk_g2s(lat2_smem, TBL ? p.weights + (size_t)model * p.weight_stride : p.weights, (uint32_t)wf4 * 16u, bars + kMaxLayers);
   }
   for (int a = 0; a < (C1 != 0 ? 2 : 1); a++)
   {
@@ -456,7 +457,7 @@ __global__ void __launch_bounds__(128 * FW, 1) wavenet_lat2_kernel(const __grid_
     y = ho1[0];
   }
   if (c.g == 0 && c.f < c.n)
-    p.out[(size_t)stream * p.out_stride + c.f] = p.head_scale * y; // model.cpp:888-897
+    p.out[(size_t)stream * p.out_stride + c.f] = (TBL && p.head_scales ? p.head_scales[model] : p.head_scale) * y; // model.cpp:888-897
   if (p.done_flag != nullptr)
   {
     // barrier, then ONE system-scope fence by the signalling thread (fences are cumulative: it orders every output store the

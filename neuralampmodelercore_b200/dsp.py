@@ -458,6 +458,36 @@ class DSP:
         self._check(self._lib.nam_b200_import_streams_device(self._h, self._i32p(s), len(s), C.c_void_p(src_ptr), stride,
                                                              C.c_void_p(cuda_stream) if cuda_stream else None))
 
+    # ---- model banks (nam_b200_create_bank_*) --------------------------------------------------------------------------
+    @property
+    def bank_size(self) -> int:
+        """K of a bank (get_dsp_bank); 1 for an ordinary handle."""
+        n = int(self._lib.nam_b200_bank_size(self._h))
+        if n < 0:
+            _raise(n, self._lib)
+        return n
+
+    def assign_streams(self, streams, models) -> None:
+        """Bind streams[i] to model models[i] and give it that model's freshly reset state; other streams are untouched.
+        On an ordinary handle, models all 0 is reset_streams."""
+        s = self._streams(streams)
+        k = np.ascontiguousarray(np.broadcast_to(np.asarray(models, dtype=np.int32), s.shape), dtype=np.int32)
+        self._check(self._lib.nam_b200_assign_streams(self._h, self._i32p(s), len(s), self._i32p(k)))
+
+    def stream_models(self, streams) -> np.ndarray:
+        """The model each listed stream is bound to (int32 array)."""
+        s = self._streams(streams)
+        out = np.zeros(len(s), np.int32)
+        self._check(self._lib.nam_b200_stream_models(self._h, self._i32p(s), len(s), self._i32p(out)))
+        return out
+
+    def model_info(self, k: int) -> _capi.Info:
+        """get_info with model k's loudness, levels, expected sample rate and weight count."""
+        info = _capi.Info()
+        info.struct_size = C.sizeof(_capi.Info)
+        self._check(self._lib.nam_b200_bank_model_info(self._h, int(k), C.byref(info)))
+        return info
+
 
 def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: Optional[bool], ctas_per_sm: int,
              kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0):
@@ -498,6 +528,54 @@ def get_dsp(config, batch: int = 1, device: int = -1, prewarm: Optional[bool] = 
     if rc != 0:
         _raise(rc, lib)
     return DSP(h.value, lib, int(batch))
+
+
+def _documents(configs) -> list:
+    """.nam paths, dicts or JSON texts -> JSON texts"""
+    import json
+
+    out = []
+    for c in configs:
+        if isinstance(c, (str, os.PathLike)) and not (isinstance(c, str) and c.lstrip().startswith("{")):
+            out.append(Path(c).read_text())
+        else:
+            out.append(c if isinstance(c, str) else json.dumps(c))
+    return out
+
+
+def _text_array(texts: list):
+    enc = [t.encode() for t in texts]
+    return (C.c_char_p * max(len(enc), 1))(*enc), enc
+
+
+def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bool] = None,
+                 fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
+                 tile_mode: int = 0, jit: int = 0) -> DSP:
+    """A model bank: one handle of `batch` streams over the K documents in `configs` (paths, dicts or JSON texts), which
+    must share one shape (bank_check).  Every stream starts bound to model 0; DSP.assign_streams rebinds.  The options are
+    get_dsp's; jit = 1 is refused for K >= 2, and a bank of one document is get_dsp."""
+    lib = _capi.load()
+    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit)
+    arr, _keep = _text_array(_documents(configs))
+    h = C.c_void_p()
+    rc = lib.nam_b200_create_bank_from_json(arr, len(_keep), C.byref(o), C.byref(h))
+    if rc != 0:
+        _raise(rc, lib)
+    return DSP(h.value, lib, int(batch))
+
+
+def bank_check(configs) -> dict:
+    """Host-only: can these documents share a bank?  {ok, n_models, reason (first offending model and field),
+    fingerprints (each model's state record fingerprint)}.  Needs no GPU."""
+    import json
+
+    lib = _capi.load()
+    arr, keep = _text_array(_documents(configs))
+    buf = C.create_string_buffer(1 << 16)
+    rc = lib.nam_b200_bank_check_json(arr, len(keep), buf, len(buf))
+    if rc != 0:
+        _raise(rc, lib)
+    return json.loads(buf.value.decode())
 
 
 def jit_prepare(config, fast_tanh: Optional[bool] = None, batch: int = 1) -> dict:
