@@ -62,6 +62,7 @@ def embed_spec_source() -> None:
     for stem in ("wavenet_spec", "lstm_spec", "wavenet_lat", "wavenet_generic_spec"):
         _embed(stem)
     _embed("generic_desc", ".h")
+    _embed("jit_params", ".h")
 
 
 def _embed(stem: str, ext: str = ".cuh") -> Path:

@@ -9,32 +9,10 @@
 // exact zeros to the sums); one CTA per stream, one thread per frame of a 128-frame tile, layer by layer.
 #pragma once
 
-#ifdef __CUDACC_RTC__ // (NVRTC: no system headers; the specialised general kernel includes this file)
-typedef unsigned int uint32_t;
-#else
-#include <stdint.h>
-#endif
+#include "jit_params.h" // StreamRef, uint32_t (the specialised general kernel includes this file under NVRTC)
 
 namespace namb200
 {
-
-// One stream of a launch that addresses streams through a table: the state row it uses and the clock at which that row's
-// history ends.  The process kernels' slot tables (position i of the call -> slots[i]) and the pack / unpack launches of
-// stream_state.cuh share it; the NVRTC-compiled kernels declare a layout twin (SlotRef).
-struct StreamRef
-{
-  int stream;
-  uint32_t clock; // the handle clock at which the stream's history ends (pack, process) or will end (unpack)
-  union
-  {
-    int alt; // Linear: the stream's history is in the alternate buffer of the double buffer
-    int model; // fused WaveNet family: the model of a bank (nam_b200_create_bank_*) this position runs; 0 otherwise
-  };
-  // process calls: frames this position runs, in [0, n_frames] of the launch (n_frames is the buffers' frame pitch).  A
-  // position stops at its own count: frames past it are neither read nor written, and a stream with 0 keeps its state.
-  // Pack / unpack launches ignore it.
-  int frames;
-};
 
 constexpr int kGenMaxVec = 64; // widest per-frame vector (channels, 2 x bottleneck, condition, head sizes)
 constexpr int kGenMaxArrays = 4;

@@ -40,6 +40,9 @@ const char* const kGenericSpecKernelSource =
 const char* const kGenericDescSource =
 #include "generic_desc_src.inc"
   ;
+const char* const kJitParamsSource =
+#include "jit_params_src.inc"
+  ;
 
 // ---- NVRTC through dlopen ------------------------------------------------------------------------------------------
 typedef struct _nvrtcProgram* nvrtcProgram;
@@ -191,11 +194,13 @@ struct CompiledKernel
 };
 
 // header + `#include "<kernel_file>"` -> sm_90a cubin, through the disk cache.  `env_override`: development aid, an
-// environment variable that names a file to use instead of the embedded kernel source.
+// environment variable that names a file to use instead of the embedded kernel source.  Every program gets jit_params.h
+// (the kernels' parameter layouts) besides `extra_headers`, and every header is part of the cache key.
 CompiledKernel compile_or_fetch(const std::string& tag, const std::string& header, const char* kernel_file,
                                 const char* embedded_source, const char* env_override, const std::vector<std::string>& defines,
-                                const std::vector<std::pair<const char*, const char*>>& extra_headers = {})
+                                std::vector<std::pair<const char*, const char*>> extra_headers = {})
 {
+  extra_headers.insert(extra_headers.begin(), {"jit_params.h", kJitParamsSource});
   CompiledKernel r;
   std::string kernel_source = embedded_source;
   if (const char* e = std::getenv(env_override))
@@ -304,7 +309,7 @@ bool spec_eligible(const WaveNetPlan& plan, const SpecGeometry& g, std::string* 
   for (float v : plan.blob)
     if (!std::isfinite(v))
       return no("non-finite weight");
-  const size_t smem = (size_t)pmax * (size_t)(plan.max_lookback + g.tile()) * 16;
+  const size_t smem = (size_t)pmax * (size_t)(plan.max_lookback + g.nt) * 16;
   if (smem * (size_t)g.min_ctas > 226u * 1024u || smem > 226u * 1024u)
     return no("history window (" + std::to_string(plan.max_lookback) + " columns) + tile do not fit in shared memory");
   return true;
@@ -367,11 +372,10 @@ SpecBuild build_spec_kernel(const WaveNetPlan& plan, const SpecGeometry& g)
     r.max_planes = std::max(r.max_planes, plan.cp[a] / 4);
 
   const std::string header = spec_header_source(plan);
-  std::vector<std::string> defs = {"-DNAMB200_SPEC_NT=" + std::to_string(g.nt), "-DNAMB200_SPEC_S=" + std::to_string(g.s),
-                                   "-DNAMB200_SPEC_MINB=" + std::to_string(g.min_ctas)};
+  std::vector<std::string> defs = {"-DNAMB200_SPEC_NT=" + std::to_string(g.nt), "-DNAMB200_SPEC_MINB=" + std::to_string(g.min_ctas)};
   // second entry point of the same cubin: the short-call variant (nt / 64 streams x 64 frames per CTA) for models
   // without a convolutional head
-  r.has_short = g.s == 1 && g.nt % 64 == 0;
+  r.has_short = g.nt % 64 == 0;
   for (int a = 0; a < plan.n_arrays; a++)
     r.has_short = r.has_short && plan.arrays[a].head_kernel == 1;
   // Two programs compiled side by side (NVRTC is re-entrant): the throughput kernel with the 64-frame short-call variant, and the
@@ -440,7 +444,6 @@ SpecBuild build_lat_kernel(const WaveNetPlan& plan, int frame_warps)
   if (32 * groups * frame_warps > 1024)
     groups = 4;
   r.geom.nt = 32 * groups * frame_warps;
-  r.geom.s = 1;
   r.geom.min_ctas = 1;
   SpecGeometry tiny; // eligibility of the family (heads, finiteness); the throughput kernel's shared-memory rule does not apply
   tiny.nt = 32;

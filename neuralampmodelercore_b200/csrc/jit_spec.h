@@ -18,12 +18,10 @@ namespace namb200
 
 struct SpecGeometry
 {
-  int nt = 512; // threads per CTA
-  int s = 1; // frames per thread
+  int nt = 512; // threads per CTA == frames per tile (one frame per thread)
   int min_ctas = 2; // __launch_bounds__ second argument
   int short_streams = 8; // streams per CTA of the short-call entry point (64 frames each)
   int short128_streams = 4, short256_streams = 2; // ... of the entry points for calls of up to 128 / 256 frames
-  int tile() const { return nt * s; }
 };
 
 struct SpecBuild
@@ -38,7 +36,7 @@ struct SpecBuild
   bool from_cache = false;
   bool has_short = false; // the cubin also holds wavenet_spec_short{,128,256}_kernel (several streams x 64 / 128 / 256 frames per CTA)
   double compile_seconds = 0.0;
-  size_t smem_bytes() const { return (size_t)max_planes * (size_t)(staged_cols + geom.tile()) * 16; }
+  size_t smem_bytes() const { return (size_t)max_planes * (size_t)(staged_cols + geom.nt) * 16; }
 };
 
 /// Can wavenet_spec.cuh serve this plan?  (The plan must already be eligible for the generic fused kernel.)

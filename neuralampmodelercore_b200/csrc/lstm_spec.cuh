@@ -21,33 +21,14 @@
 #error "include the generated model header (namespace spec) before lstm_spec.cuh"
 #endif
 
+#include "jit_params.h"
+
 namespace namb200_lstm_spec
 {
-
-// layout twin of namb200::StreamRef (generic_desc.h): one entry of a call's slot table (an LSTM has no clock)
-struct SlotRef
-{
-  int stream;
-  unsigned clock;
-  int alt;
-  int frames; // frames position b runs, <= n_frames
-};
-
-struct LstmSpecParams
-{
-  float* state; // [batch][state_stride]
-  long state_stride;
-  const float* in; // [batch][in_stride]
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  // slot table (nullptr: position b is state row b and runs n_frames frames): position b uses row slots[b].stream and
-  // runs slots[b].frames frames; inputs and outputs stay indexed by position
-  const SlotRef* slots;
-};
+using namb200::JitParams; // (an LSTM has no clock: t_base and slots[].clock are not read)
 
 // frames position `stream` runs (0 beyond the batch)
-__device__ __forceinline__ int position_frames(const LstmSpecParams& p, int stream)
+__device__ __forceinline__ int position_frames(const JitParams& p, int stream)
 {
   if (stream >= p.batch)
     return 0;
@@ -98,7 +79,7 @@ __host__ __device__ constexpr int layer_offset(int l)
 }
 
 template <bool FAST>
-__device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
+__device__ __forceinline__ void lstm_spec_body(const JitParams& p)
 {
   constexpr int H = spec::H, L = spec::L, I = spec::I;
   static_assert(I == 1, "mono models");
@@ -240,7 +221,7 @@ __device__ __forceinline__ void lstm_spec_body(const LstmSpecParams& p)
 // activation; the 4H activated values are exchanged by shuffles and every lane updates (c, h) of all units redundantly,
 // so nothing has to be broadcast back: ~115 instructions per lane per step, 8 streams per warp.
 template <bool FAST>
-__device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
+__device__ __forceinline__ void lstm_gate_split_body(const JitParams& p)
 {
   constexpr int H = spec::H, L = spec::L, I = spec::I;
   static_assert(I == 1, "mono models");
@@ -390,20 +371,20 @@ __device__ __forceinline__ void lstm_gate_split_body(const LstmSpecParams& p)
 
 } // namespace namb200_lstm_spec
 
-extern "C" __global__ void __launch_bounds__(32) lstm_spec_kernel_exact(const __grid_constant__ namb200_lstm_spec::LstmSpecParams p)
+extern "C" __global__ void __launch_bounds__(32) lstm_spec_kernel_exact(const __grid_constant__ namb200::JitParams p)
 {
   namb200_lstm_spec::lstm_spec_body<false>(p);
 }
-extern "C" __global__ void __launch_bounds__(32) lstm_spec_kernel_fast(const __grid_constant__ namb200_lstm_spec::LstmSpecParams p)
+extern "C" __global__ void __launch_bounds__(32) lstm_spec_kernel_fast(const __grid_constant__ namb200::JitParams p)
 {
   namb200_lstm_spec::lstm_spec_body<true>(p);
 }
 // gate-split variants: 8 streams per 32-thread CTA
-extern "C" __global__ void __launch_bounds__(32) lstm_spec_gates_kernel_exact(const __grid_constant__ namb200_lstm_spec::LstmSpecParams p)
+extern "C" __global__ void __launch_bounds__(32) lstm_spec_gates_kernel_exact(const __grid_constant__ namb200::JitParams p)
 {
   namb200_lstm_spec::lstm_gate_split_body<false>(p);
 }
-extern "C" __global__ void __launch_bounds__(32) lstm_spec_gates_kernel_fast(const __grid_constant__ namb200_lstm_spec::LstmSpecParams p)
+extern "C" __global__ void __launch_bounds__(32) lstm_spec_gates_kernel_fast(const __grid_constant__ namb200::JitParams p)
 {
   namb200_lstm_spec::lstm_gate_split_body<true>(p);
 }

@@ -376,6 +376,59 @@ __global__ void __launch_bounds__(256) fma_peak_kernel(float* out, int iters, fl
     out[0] = s;
 }
 
+// A module the handle compiled at run time (jit_spec.cpp), loaded from its cubin: unloaded when its owner goes away or
+// loads another one.
+class JitModule
+{
+public:
+  JitModule() = default;
+  JitModule(const JitModule&) = delete;
+  JitModule& operator=(const JitModule&) = delete;
+  ~JitModule() { unload(); }
+  explicit operator bool() const { return lib_ != nullptr; }
+  void unload()
+  {
+    if (lib_)
+      cudaLibraryUnload(lib_);
+    lib_ = nullptr;
+  }
+  // Loads `cubin` in place of the module held.  Returns "" or what failed.
+  std::string load(const std::vector<char>& cubin)
+  {
+    unload();
+    const cudaError_t e = cudaLibraryLoadData(&lib_, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+    if (e != cudaSuccess)
+      lib_ = nullptr;
+    return failed(e, "cudaLibraryLoadData");
+  }
+  // Entry point `name` -> *k, allowed `smem` bytes of dynamic shared memory (0: none); with `ctas_per_sm`, also its
+  // resident CTAs of `threads` threads per SM.  Returns "" or what failed (*k = nullptr).
+  std::string kernel(cudaKernel_t* k, const char* name, size_t smem = 0, int threads = 0, int* ctas_per_sm = nullptr) const
+  {
+    std::string why = failed(cudaLibraryGetKernel(k, lib_, name), "cudaLibraryGetKernel");
+    if (why.empty() && smem > 0)
+      why = failed(cudaFuncSetAttribute((const void*)*k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                   "cudaFuncSetAttribute");
+    if (why.empty() && ctas_per_sm)
+      why = failed(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, (const void*)*k, threads, smem),
+                   "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+    if (!why.empty())
+      *k = nullptr;
+    return why;
+  }
+
+private:
+  // "" or "<call> failed: <error>".  The error is cleared, so that a later launch check does not report it.
+  static std::string failed(cudaError_t e, const char* call)
+  {
+    if (e == cudaSuccess)
+      return "";
+    cudaGetLastError();
+    return std::string(call) + " failed: " + cudaGetErrorString(e);
+  }
+  cudaLibrary_t lib_ = nullptr;
+};
+
 } // namespace
 
 // =================================================================================================
@@ -411,8 +464,8 @@ struct nam_b200_model
   int wn_ctas_short[2] = {0, 0}; // same for the short-call (multi-stream tile) geometries 2 / 3
   int wn_geometry = 1; // 0 / 1: index into kWnGeom (FFMA kernel)
   // model-specialised kernel (wavenet_spec.cuh compiled for this model by NVRTC, jit_spec.cpp): the throughput path
-  cudaLibrary_t spec_lib = nullptr;
-  cudaLibrary_t spec_lib_extra = nullptr; // second program of the model: the 128- / 256-frame short-call entry points
+  JitModule spec_lib; // (or the LSTM's, or the general kernel's)
+  JitModule spec_lib_extra; // second program of the model: the 128- / 256-frame short-call entry points
   cudaKernel_t spec_kernel = nullptr;
   struct SpecShort // its short-call entry points (q streams x fq frames per CTA; fq = 64, 128, 256), may be absent
   {
@@ -424,7 +477,7 @@ struct nam_b200_model
   cudaKernel_t lstm_spec_kernels[2] = {nullptr, nullptr}; // lstm_spec.cuh: exact / fast activation regime
   cudaKernel_t lstm_gate_kernels[2] = {nullptr, nullptr}; // its gate-split variant (four lanes per stream)
   // low-latency kernel (wavenet_lat.cuh): few streams x short calls; built by reset() for the handle's maxBufferSize
-  cudaLibrary_t lat_lib = nullptr;
+  JitModule lat_lib;
   cudaKernel_t lat_kernel = nullptr;
   int lat_frames = 0, lat_threads = 0; // calls of up to lat_frames frames
   size_t lat_smem = 0;
@@ -515,12 +568,6 @@ struct nam_b200_model
       cudaFree(d_weights);
     if (d_glayers)
       cudaFree(d_glayers);
-    if (spec_lib)
-      cudaLibraryUnload(spec_lib);
-    if (spec_lib_extra)
-      cudaLibraryUnload(spec_lib_extra);
-    if (lat_lib)
-      cudaLibraryUnload(lat_lib);
     if (d_tile_flags)
       cudaFree(d_tile_flags);
     if (d_hist)
@@ -931,36 +978,6 @@ size_t wavenet_smem_bytes(const WaveNetPlan& plan, int geom)
 // ---- tensor-core variant dispatch ---------------------------------------------------------------
 // `stream0`: index of the handle's stream that d_in / d_out row 0 belongs to (chunked host calls)
 // ---- model-specialised kernel (wavenet_spec.cuh, compiled per model by jit_spec.cpp) ----------------------------------
-// Mirror of namb200_spec::SpecParams (wavenet_spec.cuh): the kernel's single by-value parameter.
-struct SpecKernelParams
-{
-  float* state;
-  long state_stride;
-  const float* in;
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  uint32_t t_base;
-  float* scratch; // stream-pair variant (S = 2) only: per-CTA interleaved rings; the shipped geometry is S = 1
-  long scratch_stride;
-  const StreamRef* slots; // slot table (namb200_spec::SlotRef), nullptr = rows [0, batch) at t_base; never with S = 2
-};
-
-int jit_mode(const nam_b200_model* m);
-
-struct GenSpecKernelParams // mirror of namb200_gspec::GParams
-{
-  float* state;
-  long state_stride;
-  const float* in;
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  unsigned t_base;
-  const StreamRef* slots;
-};
-
-
 // Geometry of the specialised kernel for a handle of `max_batch` streams.  Streams per CTA of the short-call entry point:
 // the count that fills whole waves of 2 CTAs per SM best (4096 streams on 132 SMs: 8 per CTA = 512 CTAs = 1.94 waves, 7 per
 // CTA = 586 = 2.22 waves).
@@ -987,91 +1004,6 @@ SpecGeometry spec_geometry_for(int max_batch, int sm_count)
   return g;
 }
 
-// Decide whether this handle gets a specialised kernel, build / fetch it, load it.  jit option: 0 = auto (on for
-// throughput handles: max_batch >= 256, where one compilation pays for itself within the first calls), 1 = required
-// (creation fails with the reason if it cannot be had), 2 = off.  $NAM_B200_JIT=0/1 overrides "auto".
-void setup_spec_kernel(nam_b200_model* m)
-{
-  const int mode = jit_mode(m);
-  const bool wanted = mode == 1 || ((mode == 0 || mode == 3) && m->opts.max_batch >= 256);
-  if (!wanted || m->opts.kernel_geometry != 0)
-    return;
-  const SpecGeometry g = spec_geometry_for(m->opts.max_batch, m->sm_count);
-  SpecBuild b = build_spec_kernel(m->plan, g);
-  if (!b.ok)
-  {
-    m->spec_state = -1;
-    m->spec_note = b.why_not;
-    if (mode == 1)
-      throw std::runtime_error("model-specialised kernel unavailable: " + b.why_not);
-    return;
-  }
-  auto check = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess)
-      throw CudaError(std::string(what) + " failed: " + cudaGetErrorString(e));
-  };
-  try
-  {
-    check(cudaLibraryLoadData(&m->spec_lib, b.cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData");
-    check(cudaLibraryGetKernel(&m->spec_kernel, m->spec_lib, spec_kernel_name()), "cudaLibraryGetKernel");
-    m->spec_geom = b.geom;
-    m->spec_smem = b.smem_bytes();
-    check(cudaFuncSetAttribute((const void*)m->spec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m->spec_smem),
-          "cudaFuncSetAttribute(spec kernel)");
-    int occ = 0;
-    check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void*)m->spec_kernel, b.geom.nt, m->spec_smem),
-          "cudaOccupancyMaxActiveBlocksPerMultiprocessor(spec kernel)");
-    if (occ < 1)
-      throw CudaError("the specialised kernel does not fit on an SM");
-    m->spec_ctas_per_sm = occ;
-    if (b.has_short)
-    {
-      const char* const names[3] = {"wavenet_spec_short_kernel", "wavenet_spec_short128_kernel", "wavenet_spec_short256_kernel"};
-      const int fqs[3] = {64, 128, 256}, qs[3] = {b.geom.short_streams, b.geom.short128_streams, b.geom.short256_streams};
-      if (!b.cubin_extra.empty()
-          && cudaLibraryLoadData(&m->spec_lib_extra, b.cubin_extra.data(), nullptr, nullptr, 0, nullptr, nullptr, 0) != cudaSuccess)
-        m->spec_lib_extra = nullptr;
-      for (int v = 0; v < 3; v++)
-      {
-        nam_b200_model::SpecShort& sv = m->spec_short[v];
-        sv = nam_b200_model::SpecShort{};
-        cudaLibrary_t lib = (v == 0) ? m->spec_lib : m->spec_lib_extra;
-        if (lib == nullptr || cudaLibraryGetKernel(&sv.kernel, lib, names[v]) != cudaSuccess)
-        {
-          sv.kernel = nullptr;
-          continue;
-        }
-        sv.fq = fqs[v];
-        sv.q = qs[v];
-        sv.smem = (size_t)b.max_planes * sv.fq * sv.q * 16;
-        if (cudaFuncSetAttribute((const void*)sv.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv.smem) != cudaSuccess
-            || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sv.ctas_per_sm, (const void*)sv.kernel, sv.fq * sv.q, sv.smem)
-                 != cudaSuccess
-            || sv.ctas_per_sm < 1)
-          sv.kernel = nullptr;
-      }
-    }
-    cudaGetLastError();
-    m->spec_state = 1;
-    m->spec_note = b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s";
-  }
-  catch (const CudaError& ex)
-  {
-    if (m->spec_lib)
-      cudaLibraryUnload(m->spec_lib);
-    if (m->spec_lib_extra)
-      cudaLibraryUnload(m->spec_lib_extra);
-    m->spec_lib = m->spec_lib_extra = nullptr;
-    for (auto& sv : m->spec_short)
-      sv = nam_b200_model::SpecShort{};
-    m->spec_kernel = nullptr;
-    m->spec_state = -1;
-    m->spec_note = ex.what();
-    if (mode == 1)
-      throw;
-  }
-}
-
 // the handle's JIT mode with the environment override applied: 1 required, 2 off, 3 preferred (try, fall back silently),
 // 0 automatic
 int jit_mode(const nam_b200_model* m)
@@ -1086,22 +1018,82 @@ int jit_mode(const nam_b200_model* m)
   return mode;
 }
 
-struct LatKernelParams // mirror of namb200_lat::LatParams
+// Does this handle want a model-specialised throughput kernel?  Required (jit = 1), or automatic / preferred on a throughput
+// handle (max_batch >= 256), where one compilation pays for itself within the first calls.  $NAM_B200_JIT=0/1 overrides
+// "automatic".
+bool jit_wanted(const nam_b200_model* m)
 {
-  float* state;
-  long state_stride;
-  const float* in;
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  uint32_t t_base;
-  unsigned* done_flag;
-  unsigned seq;
-  const StreamRef* slots;
-};
+  const int mode = jit_mode(m);
+  return mode == 1 || ((mode == 0 || mode == 3) && m->opts.max_batch >= 256);
+}
+
+// The wanted model-specialised kernel cannot be had (`why`): the handle runs the precompiled kernels and its note says why.
+// jit = 1 fails creation instead: NAM_B200_ERR_MODEL when the kernel did not compile, NAM_B200_ERR_CUDA when it did not load.
+void jit_unavailable(nam_b200_model* m, const std::string& why, bool compiled)
+{
+  m->spec_lib.unload();
+  m->spec_lib_extra.unload();
+  m->spec_kernel = m->gen_spec_kernel = nullptr;
+  for (auto& sv : m->spec_short)
+    sv = nam_b200_model::SpecShort{};
+  m->spec_state = -1;
+  m->spec_note = why;
+  if (jit_mode(m) == 1)
+  {
+    if (!compiled)
+      throw std::runtime_error("model-specialised kernel unavailable: " + why);
+    throw CudaError(why);
+  }
+}
+
+std::string jit_loaded_note(const SpecBuild& b)
+{
+  return b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s";
+}
+
+// The fused WaveNet family's specialised kernel (wavenet_spec.cuh), for handles with the default kernel geometry.  Its
+// short-call entry points are optional: one that does not load only leaves its calls to the other kernels.
+void setup_spec_kernel(nam_b200_model* m)
+{
+  if (!jit_wanted(m) || m->opts.kernel_geometry != 0)
+    return;
+  const SpecBuild b = build_spec_kernel(m->plan, spec_geometry_for(m->opts.max_batch, m->sm_count));
+  m->spec_geom = b.geom;
+  m->spec_smem = b.smem_bytes();
+  std::string why = b.ok ? m->spec_lib.load(b.cubin) : b.why_not;
+  if (why.empty())
+    why = m->spec_lib.kernel(&m->spec_kernel, spec_kernel_name(), m->spec_smem, b.geom.nt, &m->spec_ctas_per_sm);
+  if (why.empty() && m->spec_ctas_per_sm < 1)
+    why = "the specialised kernel does not fit on an SM";
+  if (!why.empty())
+    return jit_unavailable(m, why, b.ok);
+  if (b.has_short)
+  {
+    const char* const names[3] = {"wavenet_spec_short_kernel", "wavenet_spec_short128_kernel", "wavenet_spec_short256_kernel"};
+    const int fqs[3] = {64, 128, 256}, qs[3] = {b.geom.short_streams, b.geom.short128_streams, b.geom.short256_streams};
+    if (!b.cubin_extra.empty())
+      m->spec_lib_extra.load(b.cubin_extra);
+    for (int v = 0; v < 3; v++)
+    {
+      nam_b200_model::SpecShort& sv = m->spec_short[v];
+      sv = nam_b200_model::SpecShort{};
+      const JitModule& lib = (v == 0) ? m->spec_lib : m->spec_lib_extra;
+      if (!lib)
+        continue;
+      sv.fq = fqs[v];
+      sv.q = qs[v];
+      sv.smem = (size_t)b.max_planes * sv.fq * sv.q * 16;
+      if (!lib.kernel(&sv.kernel, names[v], sv.smem, sv.fq * sv.q, &sv.ctas_per_sm).empty() || sv.ctas_per_sm < 1)
+        sv.kernel = nullptr;
+    }
+  }
+  m->spec_state = 1;
+  m->spec_note = jit_loaded_note(b);
+}
 
 // reset(): plugin-style handles (few streams, maxBufferSize <= 128) get the low-latency kernel for calls of up to
 // 64 / 128 frames.  Wanted when jit is "required" or "preferred" (the C++ shim's default), never by the automatic policy.
+// It never fails creation: without it the precompiled short-call geometries serve the handle.
 void setup_lat_kernel(nam_b200_model* m)
 {
   if (m->spec.arch != Arch::WaveNet || m->use_generic || m->opts.kernel_geometry != 0)
@@ -1112,67 +1104,55 @@ void setup_lat_kernel(nam_b200_model* m)
   const int fw = m->max_frames <= 64 ? 2 : 4;
   if (m->lat_state == 1 && m->lat_frames == 32 * fw)
     return;
-  if (m->lat_lib)
-    cudaLibraryUnload(m->lat_lib);
-  m->lat_lib = nullptr;
-  m->lat_kernel = nullptr;
-  m->lat_state = 0;
-  SpecBuild b = build_lat_kernel(m->plan, fw);
-  if (!b.ok)
-  {
-    m->lat_state = -1;
-    m->lat_note = b.why_not;
-    return; // the precompiled short-call geometries serve the handle
-  }
-  cudaError_t e = cudaLibraryLoadData(&m->lat_lib, b.cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-  if (e == cudaSuccess)
-    e = cudaLibraryGetKernel(&m->lat_kernel, m->lat_lib, "wavenet_lat_kernel");
+  const SpecBuild b = build_lat_kernel(m->plan, fw);
   m->lat_smem = lat_smem_bytes(m->plan, 32 * fw);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute((const void*)m->lat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m->lat_smem);
-  if (e != cudaSuccess)
+  std::string why = b.why_not;
+  if (b.ok)
   {
-    cudaGetLastError();
-    if (m->lat_lib)
-      cudaLibraryUnload(m->lat_lib);
-    m->lat_lib = nullptr;
+    std::string err = m->lat_lib.load(b.cubin);
+    if (err.empty())
+      err = m->lat_lib.kernel(&m->lat_kernel, "wavenet_lat_kernel", m->lat_smem);
+    if (!err.empty())
+      why = "loading the low-latency kernel failed: " + err;
+  }
+  if (!why.empty())
+  {
+    m->lat_lib.unload();
     m->lat_kernel = nullptr;
     m->lat_state = -1;
-    m->lat_note = std::string("loading the low-latency kernel failed: ") + cudaGetErrorString(e);
+    m->lat_note = why;
     return;
   }
-  if (!m->h_flag && cudaHostAlloc(&m->h_flag, 64, cudaHostAllocMapped) == cudaSuccess)
-  {
-    *m->h_flag = 0;
-    if (cudaHostGetDevicePointer(&m->h_flag_dev, m->h_flag, 0) != cudaSuccess)
-      m->h_flag_dev = nullptr;
-  }
-  cudaGetLastError();
   m->lat_frames = 32 * fw;
   m->lat_threads = b.geom.nt;
   m->lat_state = 1;
-  m->lat_note = b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s";
+  m->lat_note = jit_loaded_note(b);
 }
 
-void launch_wavenet_lat(nam_b200_model* m, const WaveNetKernelParams& kp, cudaStream_t st)
+// The parameter of the model-specialised kernels for one call: rows from `state` (the table's rows when `slots`), the call's
+// buffers, strides, batch and frames, at the handle's clock
+JitParams jit_params(const nam_b200_model* m, float* state, const float* d_in, float* d_out, long in_stride, long out_stride,
+                     int batch, int n_frames, const StreamRef* slots)
+{
+  return JitParams{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, m->t_base, slots};
+}
+
+void launch_wavenet_lat(nam_b200_model* m, const JitParams& jp, cudaStream_t st)
 {
   // single-stream calls ring the doorbell in mapped host memory (process_planar spins on it instead of synchronising)
-  unsigned* flag = (kp.batch == 1 && m->h_flag_dev != nullptr) ? m->h_flag_dev : nullptr;
+  unsigned* flag = (jp.batch == 1 && m->h_flag_dev != nullptr) ? m->h_flag_dev : nullptr;
   if (flag)
     m->flag_seq++;
-  LatKernelParams lp{kp.state, kp.state_stride, kp.in, kp.out, kp.in_stride, kp.out_stride, kp.batch, kp.n_frames, kp.t_base,
-                     flag, m->flag_seq, kp.slots};
+  LatParams lp{jp, flag, m->flag_seq};
   m->flag_pending = flag != nullptr;
   void* args[] = {&lp};
-  CUDA_CHECK(cudaLaunchKernel((const void*)m->lat_kernel, dim3(kp.batch), dim3(m->lat_threads), args, m->lat_smem, st));
+  CUDA_CHECK(cudaLaunchKernel((const void*)m->lat_kernel, dim3(jp.batch), dim3(m->lat_threads), args, m->lat_smem, st));
 }
 
-void launch_wavenet_spec(nam_b200_model* m, const WaveNetKernelParams& kp, cudaStream_t st)
+void launch_wavenet_spec(nam_b200_model* m, JitParams jp, cudaStream_t st)
 {
-  SpecKernelParams sp{kp.state, kp.state_stride, kp.in,  kp.out, kp.in_stride, kp.out_stride,
-                      kp.batch, kp.n_frames,     kp.t_base, nullptr, 0, kp.slots};
-  void* args[] = {&sp};
-  int grid = std::min(kp.batch, m->spec_ctas_per_sm * std::max(1, m->sm_count - m->reserved_sms));
+  void* args[] = {&jp};
+  int grid = std::min(jp.batch, m->spec_ctas_per_sm * std::max(1, m->sm_count - m->reserved_sms));
   if (grid < 1)
     grid = 1;
   CUDA_CHECK(cudaLaunchKernel((const void*)m->spec_kernel, dim3(grid), dim3(m->spec_geom.nt), args, m->spec_smem, st));
@@ -1183,10 +1163,10 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
                     long out_stride, cudaStream_t st, int stream0 = 0, const StreamRef* slots = nullptr)
 {
   float* const state0 = slots ? m->d_state : m->d_state + (size_t)stream0 * (size_t)m->state_stride;
+  JitParams jp = jit_params(m, state0, d_in, d_out, in_stride, out_stride, batch, n_frames, slots);
   if (m->use_generic && m->gen_spec_kernel != nullptr && m->opts.kernel_geometry == 0)
   {
-    GenSpecKernelParams sp{state0, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, m->t_base, slots};
-    void* args[] = {&sp};
+    void* args[] = {&jp};
     CUDA_CHECK(cudaLaunchKernel((const void*)m->gen_spec_kernel, dim3(std::max(1, std::min(batch, 16 * m->sm_count))), dim3(kGenTile),
                                 args, 0, st));
     m->launches++;
@@ -1275,7 +1255,7 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
     if (jit_lat_ok)
     {
       // the model-specialised variant (wavenet_lat.cuh)
-      launch_wavenet_lat(m, kp, st);
+      launch_wavenet_lat(m, jp, st);
       m->launches++;
       return;
     }
@@ -1288,15 +1268,11 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
         continue;
       if (sv.kernel == nullptr || batch < 2 * sv.q)
         break; // the smallest variant that holds the call, or none
-      {
-        SpecKernelParams sp{kp.state, kp.state_stride, kp.in,  kp.out, kp.in_stride, kp.out_stride,
-                            kp.batch, kp.n_frames,     kp.t_base, nullptr, 0, kp.slots};
-        void* args[] = {&sp};
-        const int grid_s = std::max(1, std::min((batch + sv.q - 1) / sv.q, sv.ctas_per_sm * m->sm_count));
-        CUDA_CHECK(cudaLaunchKernel((const void*)sv.kernel, dim3(grid_s), dim3(sv.fq * sv.q), args, sv.smem, st));
-        m->launches++;
-        return;
-      }
+      void* args[] = {&jp};
+      const int grid_s = std::max(1, std::min((batch + sv.q - 1) / sv.q, sv.ctas_per_sm * m->sm_count));
+      CUDA_CHECK(cudaLaunchKernel((const void*)sv.kernel, dim3(grid_s), dim3(sv.fq * sv.q), args, sv.smem, st));
+      m->launches++;
+      return;
     }
   // short calls on more than a handful of streams: several streams per tile (same rings, same arithmetic)
   for (int sg = 0; sg < 2; sg++)
@@ -1384,10 +1360,9 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
       return;
     }
   }
-  // (the stream-pair variant, S = 2, takes no slot table: such calls run the fused kernel below)
-  if (m->spec_state == 1 && m->opts.kernel_geometry == 0 && !(slots && m->spec_geom.s == 2))
+  if (m->spec_state == 1 && m->opts.kernel_geometry == 0)
   {
-    launch_wavenet_spec(m, kp, st);
+    launch_wavenet_spec(m, jp, st);
     m->launches++;
     return;
   }
@@ -1399,86 +1374,43 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
 }
 
 // ---- model-specialised LSTM kernel (lstm_spec.cuh through jit_spec.cpp): same policy as setup_spec_kernel ------------
-struct LstmSpecKernelParams // mirror of namb200_lstm_spec::LstmSpecParams
-{
-  float* state;
-  long state_stride;
-  const float* in;
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  const StreamRef* slots;
-};
-
 void setup_lstm_spec_kernel(nam_b200_model* m)
 {
-  const int mode = jit_mode(m);
-  if (!(mode == 1 || ((mode == 0 || mode == 3) && m->opts.max_batch >= 256)))
+  if (!jit_wanted(m))
     return;
-  SpecBuild b = build_lstm_spec_kernel(m->spec);
-  if (!b.ok)
-  {
-    m->spec_state = -1;
-    m->spec_note = b.why_not;
-    if (mode == 1)
-      throw std::runtime_error("model-specialised kernel unavailable: " + b.why_not);
-    return;
-  }
-  auto check = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess)
-      throw CudaError(std::string(what) + " failed: " + cudaGetErrorString(e));
-  };
-  try
-  {
-    check(cudaLibraryLoadData(&m->spec_lib, b.cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData");
-    check(cudaLibraryGetKernel(&m->lstm_spec_kernels[0], m->spec_lib, "lstm_spec_kernel_exact"), "cudaLibraryGetKernel");
-    check(cudaLibraryGetKernel(&m->lstm_spec_kernels[1], m->spec_lib, "lstm_spec_kernel_fast"), "cudaLibraryGetKernel");
-    check(cudaLibraryGetKernel(&m->lstm_gate_kernels[0], m->spec_lib, "lstm_spec_gates_kernel_exact"), "cudaLibraryGetKernel");
-    check(cudaLibraryGetKernel(&m->lstm_gate_kernels[1], m->spec_lib, "lstm_spec_gates_kernel_fast"), "cudaLibraryGetKernel");
-    m->spec_state = 1;
-    m->spec_note = b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s";
-  }
-  catch (const CudaError& ex)
-  {
-    if (m->spec_lib)
-      cudaLibraryUnload(m->spec_lib);
-    m->spec_lib = nullptr;
-    m->spec_state = -1;
-    m->spec_note = ex.what();
-    if (mode == 1)
-      throw;
-  }
+  const SpecBuild b = build_lstm_spec_kernel(m->spec);
+  std::string why = b.ok ? m->spec_lib.load(b.cubin) : b.why_not;
+  const char* const names[4] = {"lstm_spec_kernel_exact", "lstm_spec_kernel_fast", "lstm_spec_gates_kernel_exact",
+                                "lstm_spec_gates_kernel_fast"};
+  cudaKernel_t* const kernels[4] = {&m->lstm_spec_kernels[0], &m->lstm_spec_kernels[1], &m->lstm_gate_kernels[0],
+                                    &m->lstm_gate_kernels[1]};
+  for (int i = 0; i < 4 && why.empty(); i++)
+    why = m->spec_lib.kernel(kernels[i], names[i]);
+  if (!why.empty())
+    return jit_unavailable(m, why, b.ok);
+  m->spec_state = 1;
+  m->spec_note = jit_loaded_note(b);
 }
 
 // ---- the general kernel compiled for this model (wavenet_generic_spec.cuh): same policy as the fused family's -------------
 void setup_generic_spec_kernel(nam_b200_model* m)
 {
-  const int mode = jit_mode(m);
-  if (!(mode == 1 || ((mode == 0 || mode == 3) && m->opts.max_batch >= 256)) || m->opts.kernel_geometry == 4)
+  if (!jit_wanted(m) || m->opts.kernel_geometry == 4)
     return;
-  SpecBuild b = build_generic_spec_kernel(m->gplan);
-  auto give_up = [&](const std::string& why) {
-    if (m->spec_lib)
-      cudaLibraryUnload(m->spec_lib);
-    m->spec_lib = nullptr;
-    m->gen_spec_kernel = nullptr;
-    m->spec_state = -1;
-    m->spec_note = why;
-    if (mode == 1)
-      throw std::runtime_error("model-specialised kernel unavailable: " + why);
-  };
-  if (!b.ok)
-    return give_up(b.why_not);
-  cudaError_t e = cudaLibraryLoadData(&m->spec_lib, b.cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-  if (e == cudaSuccess)
-    e = cudaLibraryGetKernel(&m->gen_spec_kernel, m->spec_lib, "wavenet_generic_spec_kernel");
-  if (e != cudaSuccess)
+  const SpecBuild b = build_generic_spec_kernel(m->gplan);
+  std::string why = b.why_not;
+  if (b.ok)
   {
-    cudaGetLastError();
-    return give_up(std::string("loading the specialised general kernel failed: ") + cudaGetErrorString(e));
+    std::string err = m->spec_lib.load(b.cubin);
+    if (err.empty())
+      err = m->spec_lib.kernel(&m->gen_spec_kernel, "wavenet_generic_spec_kernel");
+    if (!err.empty())
+      why = "loading the specialised general kernel failed: " + err;
   }
+  if (!why.empty())
+    return jit_unavailable(m, why, b.ok);
   m->spec_state = 1;
-  m->spec_note = std::string("general kernel, ") + (b.from_cache ? "cubin from cache" : "compiled in " + std::to_string(b.compile_seconds) + " s");
+  m->spec_note = "general kernel, " + jit_loaded_note(b);
 }
 
 // `state`: rows of per-stream state to run on (nullptr = the handle's d_state; nam_b200_reset_streams prewarms a gathered
@@ -1490,8 +1422,8 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
     state = m->d_state;
   if (m->spec_state == 1)
   {
-    LstmSpecKernelParams sp{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, slots};
-    void* args[] = {&sp};
+    JitParams jp = jit_params(m, state, d_in, d_out, in_stride, out_stride, batch, n_frames, slots);
+    void* args[] = {&jp};
     // The step rate is bound by one warp's instruction stream as long as every warp has a scheduler to itself: four
     // lanes per stream (gate-split, 8 streams per warp: a shorter dependent chain per step) while every warp still gets a
     // scheduler of its own (4 x SMs), else one thread per stream (32 per warp: more streams in flight).  kernel_geometry
@@ -3103,10 +3035,10 @@ int nam_b200_jit_prepare_json_for_batch(const char* nam_json_text, int fast_tanh
     char buf[1024];
     std::snprintf(buf, sizeof buf,
                   "{\"ok\": %s, \"from_cache\": %s, \"compile_seconds\": %.3f, \"cubin_bytes\": %zu, \"threads\": %d, "
-                  "\"frames_per_thread\": %d, \"smem_bytes\": %zu, \"why_not\": \"%s\", \"lat_ok\": %s, "
+                  "\"frames_per_thread\": 1, \"smem_bytes\": %zu, \"why_not\": \"%s\", \"lat_ok\": %s, "
                   "\"lat_compile_seconds\": %.3f, \"lat_cubin_bytes\": %zu}",
                   b.ok ? "true" : "false", b.from_cache ? "true" : "false", b.compile_seconds, b.cubin.size() + b.cubin_extra.size(), b.geom.nt,
-                  b.geom.s, b.ok ? b.smem_bytes() : (size_t)0, why.c_str(), lat.ok ? "true" : "false", lat.compile_seconds,
+                  b.ok ? b.smem_bytes() : (size_t)0, why.c_str(), lat.ok ? "true" : "false", lat.compile_seconds,
                   lat.cubin.size());
     if (out && capacity > 0)
     {

@@ -80,7 +80,7 @@ struct StateChunk
   int seg, item0;
 };
 
-// one stream of a pack / unpack launch: StreamRef (generic_desc.h); `alt` is read by pack only
+// one stream of a pack / unpack launch: StreamRef (jit_params.h); `alt` is read by pack only
 static_assert(sizeof(StreamRef) == 16, "StreamRef is 16 bytes");
 
 constexpr int kStateThreads = 256;

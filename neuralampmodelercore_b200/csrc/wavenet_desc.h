@@ -4,7 +4,7 @@
 
 #include <stdint.h>
 
-#include "generic_desc.h" // StreamRef
+#include "generic_desc.h" // StreamRef (jit_params.h)
 
 namespace namb200
 {

@@ -36,20 +36,6 @@ enum : int
   ACT_SOFTSIGN = 10
 };
 
-struct GParams
-{
-  float* state; // [stream][state_stride]
-  long state_stride;
-  const float* in; // stream s, channel c: in[s * in_stride + c * n_frames ..]
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  unsigned t_base;
-  // nullptr: position s is state row s at t_base running n_frames frames; else row slots[s].stream at slots[s].clock
-  // running slots[s].frames
-  const StreamRef* slots;
-};
-
 constexpr int kTile = 128; // frames per tile == threads per CTA (the ring geometry of generic_pack.cpp assumes it)
 
 struct Th
@@ -321,7 +307,7 @@ __device__ __forceinline__ void net_forward(const Th& c, const float* in, const 
 
 } // namespace namb200_gspec
 
-extern "C" __global__ void __launch_bounds__(namb200_gspec::kTile) wavenet_generic_spec_kernel(const __grid_constant__ namb200_gspec::GParams p)
+extern "C" __global__ void __launch_bounds__(namb200_gspec::kTile) wavenet_generic_spec_kernel(const __grid_constant__ namb200::JitParams p)
 {
   using namespace namb200_gspec;
   Th c;

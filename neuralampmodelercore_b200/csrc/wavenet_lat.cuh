@@ -42,21 +42,7 @@ using namespace namb200_spec;
 constexpr int kGroups = NAMB200_LAT_GROUPS;
 static_assert(kGroups == 4 || kGroups == 8, "4 or 8 channel groups");
 
-struct LatParams
-{
-  float* state; // [batch][state_stride]
-  long state_stride;
-  const float* in; // [batch][in_stride] (may be mapped host memory)
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames; // n_frames <= 32 * FW
-  u32 t_base;
-  // completion doorbell (may be null): a word in mapped host memory that receives `seq` once every output of the call
-  // is visible to the host -- the host spins on it instead of paying a stream synchronisation per 64-frame call
-  unsigned* done_flag;
-  unsigned seq;
-  const SlotRef* slots; // as SpecParams::slots
-};
+using namb200::LatParams; // (jit_params.h; in may be mapped host memory, n_frames <= 32 * FW)
 
 // ---- shared-memory plan (float4 columns) ------------------------------------------------------------------------------
 //   tile [Pmax][F]   the current layer's input columns of this call
@@ -435,7 +421,7 @@ __device__ __forceinline__ void wavenet_lat_body(const LatParams& p)
 #endif
 
 extern "C" __global__ void __launch_bounds__(32 * NAMB200_LAT_GROUPS * NAMB200_LAT_FW, 1)
-  wavenet_lat_kernel(const __grid_constant__ namb200_lat::LatParams p)
+  wavenet_lat_kernel(const __grid_constant__ namb200::LatParams p)
 {
   namb200_lat::wavenet_lat_body<NAMB200_LAT_FW>(p);
 }

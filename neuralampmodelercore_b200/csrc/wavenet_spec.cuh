@@ -15,7 +15,7 @@
 //   activations.h:59-133 -- in the same summation order (bias + mixin first, taps oldest to newest, input channels
 //   ascending), so its results are bit-identical to the generic fused kernel's.
 //
-// Mapping: one persistent CTA owns one stream at a time and walks its call in tiles of T = S * NT frames; thread t owns
+// Mapping: one persistent CTA owns one stream at a time and walks its call in tiles of T = NT frames; thread t owns
 // frames {t, t + NT, ..} for the whole depth of the network (see wavenet_fused.cuh).  What is new here:
 //   * TMA-engine staging of the history (cp.async.bulk, SASS UBLKCP): before a layer runs, the last `lookback` columns of
 //     its input ring are copied global -> shared by bulk-async copies that complete on an mbarrier, into the columns
@@ -33,8 +33,11 @@
 #error "include the generated model header (namespace spec) before wavenet_spec.cuh"
 #endif
 
+#include "jit_params.h"
+
 namespace namb200_spec
 {
+using namb200::JitParams;
 typedef unsigned long long u64;
 typedef unsigned int u32;
 
@@ -52,32 +55,6 @@ enum : int
   ACT_HARDSWISH = 8,
   ACT_LEAKYHARDTANH = 9,
   ACT_SOFTSIGN = 10
-};
-
-// layout twin of namb200::StreamRef (generic_desc.h): one entry of a call's slot table
-struct SlotRef
-{
-  int stream; // state row of this position of the call
-  u32 clock; // where that row's history ends
-  int alt;
-  int frames; // frames this position runs, <= n_frames (the buffers' frame pitch)
-};
-
-struct SpecParams
-{
-  float* state; // [batch][state_stride]: the rings of wavenet_fused.cuh
-  long state_stride; // floats
-  const float* in; // [batch][in_stride]
-  float* out;
-  long in_stride, out_stride;
-  int batch, n_frames;
-  u32 t_base; // absolute frame index of in[:, 0] (mod 2^32)
-  float* scratch; // S = 2: [grid][scratch_stride] floats, a CTA's stream pair in the interleaved layout
-  long scratch_stride; // 2 * state_stride
-  // slot table (nullptr: position b is state row b at t_base, running n_frames frames): position b uses row slots[b].stream
-  // at slots[b].clock and runs slots[b].frames frames; inputs and outputs stay indexed by position.  The stream-pair
-  // variant (S = 2) is never given one.
-  const SlotRef* slots;
 };
 
 // ---- scalar helpers (same arithmetic as wavenet_fused.cuh) ------------------------------------------------------
@@ -149,64 +126,8 @@ __device__ __forceinline__ float act_sigmoid(float x)
   return rcp_approx(1.0f + expf(-x));
 }
 
-// ---- frame vectors -------------------------------------------------------------------------------------------------------
-// S = 1: a thread owns frame `tid` of ONE stream, V = float.
-// S = 2: a thread owns frame `tid` of a PAIR of streams (2q, 2q + 1), V = a register pair (low half = the even
-// stream).  Everything a layer does is written once over V.  The form was made for a packed FMA with a broadcast
-// immediate weight; sm_90 has none, so each pair operation is two scalar FFMAs and S = 1 is the default.  The pair must sit in an aligned register pair, so the activations of the two streams are
-// interleaved element-wise wherever they are stored: a column of a "sub-plane" is 16 bytes = (c A, c B, c' A, c' B) for
-// two channels c, c' -- one LDS.128 yields two ready pairs, conflict-free.  The rings of the library keep one stream
-// per ring ([C/4][R][4 floats]), so the kernel converts a pair's rings into a per-CTA scratch in the interleaved layout
-// when it picks the pair up, runs all tiles of the call on the scratch (bulk copies move interleaved columns), and
-// converts back at the end: other kernels never see the interleaved layout.
-template <int S>
-struct FrameVec;
-template <>
-struct FrameVec<1>
-{
-  typedef float type;
-};
-template <>
-struct FrameVec<2>
-{
-  typedef u64 type;
-};
-
-__device__ __forceinline__ float vfma(const float x, const float w, const float a)
-{
-  return fmaf(w, x, a);
-}
-__device__ __forceinline__ u64 vfma(const u64 x, const float w, const u64 a)
-{
-  return fma2(x, dup2(w), a);
-}
-__device__ __forceinline__ float vadd(const float a, const float b)
-{
-  return a + b;
-}
-__device__ __forceinline__ u64 vadd(const u64 a, const u64 b)
-{
-  return add2(a, b);
-}
-__device__ __forceinline__ float vaddc(const float a, const float c)
-{
-  return a + c;
-}
-__device__ __forceinline__ u64 vaddc(const u64 a, const float c)
-{
-  return add2(a, dup2(c));
-}
-__device__ __forceinline__ void vsplat(float& v, const float c)
-{
-  v = c;
-}
-__device__ __forceinline__ void vsplat(u64& v, const float c)
-{
-  v = dup2(c);
-}
-// The 4 channels of plane `pl` at column offset `off` behind this thread's own column.  `col0` = the thread's column in
-// (sub-)plane 0, W = columns per (sub-)plane.  S = 1: one 16-byte column of a 4-channel plane.  S = 2: two 16-byte
-// columns of two 2-channel sub-planes, each (c A, c B, c' A, c' B).
+// The 4 channels of plane `pl` at column offset `off` behind this thread's own column: one 16-byte column.  `col0` = the
+// thread's column in plane 0, W = columns per plane.
 template <int W>
 __device__ __forceinline__ void load_plane(const float4* col0, const int pl, const int off, float (&x)[4])
 {
@@ -214,22 +135,9 @@ __device__ __forceinline__ void load_plane(const float4* col0, const int pl, con
   x[0] = q.x, x[1] = q.y, x[2] = q.z, x[3] = q.w;
 }
 template <int W>
-__device__ __forceinline__ void load_plane(const float4* col0, const int pl, const int off, u64 (&x)[4])
-{
-  const float4 q0 = col0[(2 * pl) * W - off], q1 = col0[(2 * pl + 1) * W - off];
-  x[0] = pack2(q0.x, q0.y), x[1] = pack2(q0.z, q0.w), x[2] = pack2(q1.x, q1.y), x[3] = pack2(q1.z, q1.w);
-}
-template <int W>
 __device__ __forceinline__ void store_plane(float4* col0, const int pl, const float (&x)[4])
 {
   col0[pl * W] = make_float4(x[0], x[1], x[2], x[3]);
-}
-template <int W>
-__device__ __forceinline__ void store_plane(float4* col0, const int pl, const u64 (&x)[4])
-{
-  float4 q0, q1;
-  unpack2(x[0], q0.x, q0.y), unpack2(x[1], q0.z, q0.w), unpack2(x[2], q1.x, q1.y), unpack2(x[3], q1.z, q1.w);
-  col0[(2 * pl) * W] = q0, col0[(2 * pl + 1) * W] = q1;
 }
 
 // one element of layer LI's activation, channel i (activations.h:59-133)
@@ -279,22 +187,6 @@ __device__ __forceinline__ void apply_activation(float (&v)[C])
 #pragma unroll
     for (int i = 0; i < C; i++)
       v[i] = act_scalar<LI, C>(v[i], i);
-  }
-}
-template <int LI, int C>
-__device__ __forceinline__ void apply_activation(u64 (&v)[C])
-{
-#pragma unroll
-  for (int i = 0; i < C; i++)
-  {
-    if constexpr (spec::L[LI].act == ACT_FASTTANH)
-      v[i] = fast_tanh2(v[i]); // the two frames of the channel per packed operation
-    else
-    {
-      float a, b;
-      unpack2(v[i], a, b);
-      v[i] = pack2(act_scalar<LI, C>(a, i), act_scalar<LI, C>(b, i));
-    }
   }
 }
 
@@ -424,50 +316,48 @@ struct TileCtx
 };
 
 // history of the unit that follows (AI, LI) in program order is requested right after the current unit's last read
-template <int AI, int NT, int S, int LI>
+template <int AI, int NT, int LI>
 __device__ __forceinline__ void request_layer_history(TileCtx& c, IntC<LI>)
 {
   constexpr spec::Layer Ld = spec::L[LI];
   constexpr int C = spec::A[AI].C;
   constexpr int W = spec::LS + NT;
-  // S = 2: C/2 sub-planes of 16-byte columns; the interleaved ring of a pair is twice the size of one stream's ring
   if (c.warp == 0)
-    hist_load<(S == 1 ? C / 4 : C / 2), (Ld.K - 1) * Ld.dil, Ld.ring_mask, W>(c.buf, c.state + S * Ld.ring_off, c.tabs0, c.bar,
-                                                                              c.lane);
+    hist_load<C / 4, (Ld.K - 1) * Ld.dil, Ld.ring_mask, W>(c.buf, c.state + Ld.ring_off, c.tabs0, c.bar, c.lane);
 }
 
-// One layer array for the S frames a thread owns (cf. namb200::array_forward), V = FrameVec<S>.
+// One layer array for the frame a thread owns (cf. namb200::array_forward).
 //   hin[CIN]: the array's input (the raw sample for the first array, the previous array's last layer output after)
 //   head[C]: the head accumulator, initialised by the caller (zeros, or the previous array's head output)
 //   headout[HOUT]: this array's head output
 //   NEXT_AI: the array that follows (-1: none) -- its first layer's history is requested after this array's last tap read
-template <int AI, int NEXT_AI, int NT, int S, typename V>
-__device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A[AI].CIN], const V cond, V (&head)[spec::A[AI].C],
-                                              V (&hout)[spec::A[AI].C], V (&headout)[spec::A[AI].HOUT])
+template <int AI, int NEXT_AI, int NT>
+__device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spec::A[AI].CIN], const float cond,
+                                              float (&head)[spec::A[AI].C], float (&hout)[spec::A[AI].C],
+                                              float (&headout)[spec::A[AI].HOUT])
 {
   constexpr spec::Array A = spec::A[AI];
   constexpr int C = A.C, CIN = A.CIN, HOUT = A.HOUT, P = C / 4;
   constexpr int W = spec::LS + NT;
-  constexpr int HP = (S == 1) ? C / 4 : C / 2; // (sub-)planes the history copies move
   constexpr int HEADK = A.head_kernel, HRMASK = A.head_ring_mask, HROFF = A.head_ring_off;
   constexpr int HL = (A.head_kernel - 1) * A.head_dilation; // look-back of a convolutional head (0: kernel size 1)
-  float4* const col0 = c.buf + spec::LS + threadIdx.x; // this thread's column of (sub-)plane 0
+  float4* const col0 = c.buf + spec::LS + threadIdx.x; // this thread's column of plane 0
 
   // ---- rechannel (Conv1x1, no bias; model.cpp:492) -> this thread's columns of the tile
   {
-    V h[C];
+    float h[C];
 #pragma unroll
     for (int o = 0; o < C; o++)
-      vsplat(h[o], 0.0f);
+      h[o] = 0.0f;
 #pragma unroll
     for (int i = 0; i < CIN; i++)
 #pragma unroll
       for (int o = 0; o < C; o++)
-        h[o] = vfma(hin[i], spec::w(A.rech_off + i * C + o), h[o]);
+        h[o] = fmaf(spec::w(A.rech_off + i * C + o), hin[i], h[o]);
 #pragma unroll
     for (int pl = 0; pl < P; pl++)
     {
-      const V q[4] = {h[4 * pl], h[4 * pl + 1], h[4 * pl + 2], h[4 * pl + 3]};
+      const float q[4] = {h[4 * pl], h[4 * pl + 1], h[4 * pl + 2], h[4 * pl + 3]};
       store_plane<W>(col0, pl, q);
     }
   }
@@ -485,17 +375,13 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A
     mbar_wait(c.bar, c.phase); // .. and its history has landed in front of it
     c.phase ^= 1u;
     if (c.warp == 0) // newest columns -> ring (reads the tile until B1)
-      hist_store<HP, L, Ld.ring_mask, W>(c.buf, c.state + S * Ld.ring_off, c.tabs0, c.tv, c.lane);
+      hist_store<P, L, Ld.ring_mask, W>(c.buf, c.state + Ld.ring_off, c.tabs0, c.tv, c.lane);
 
     // ---- phase 1: z = b + M c + sum_k W_k h[t - (K-1-k) d];  a = act(z);  head += a
-    V acc[C];
+    float acc[C];
 #pragma unroll
     for (int o = 0; o < C; o++)
-    {
-      V b;
-      vsplat(b, spec::w(w_bias + o));
-      acc[o] = vfma(cond, spec::w(w_mix + o), b);
-    }
+      acc[o] = fmaf(spec::w(w_mix + o), cond, spec::w(w_bias + o));
 #pragma unroll
     for (int k = 0; k < K; k++)
     {
@@ -503,64 +389,55 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A
 #pragma unroll
       for (int pl = 0; pl < P; pl++)
       {
-        V x[4];
+        float x[4];
         load_plane<W>(col0, pl, off, x);
 #pragma unroll
         for (int i = 0; i < 4; i++)
 #pragma unroll
           for (int o = 0; o < C; o++)
-            acc[o] = vfma(x[i], spec::w(w_conv + (k * C + 4 * pl + i) * C + o), acc[o]);
+            acc[o] = fmaf(spec::w(w_conv + (k * C + 4 * pl + i) * C + o), x[i], acc[o]);
       }
     }
     apply_activation<LI, C>(acc);
-    if constexpr (S == 1)
-    {
 #pragma unroll
-      for (int q = 0; q < C / 2; q++) // model.cpp:530 (packed add over channel pairs: half the issue slots)
-        unpack2(add2(pack2(head[2 * q], head[2 * q + 1]), pack2(acc[2 * q], acc[2 * q + 1])), head[2 * q], head[2 * q + 1]);
-    }
-    else
-    {
-#pragma unroll
-      for (int o = 0; o < C; o++)
-        head[o] = vadd(head[o], acc[o]); // model.cpp:530
-    }
-    if (c.warp == 0 && c.lane < HP)
+    for (int q = 0; q < C / 2; q++) // model.cpp:530 (packed add over channel pairs: half the issue slots)
+      unpack2(add2(pack2(head[2 * q], head[2 * q + 1]), pack2(acc[2 * q], acc[2 * q + 1])), head[2 * q], head[2 * q + 1]);
+    if (c.warp == 0 && c.lane < P)
       bulk_wait_all(); // my ring stores are done: the tile may be rewritten, the rings may be re-read
     __syncthreads(); // B1: every tap read of this layer's input is done
     // the next unit's history lands under this layer's 1x1 phase
     if constexpr (!last)
-      request_layer_history<AI, NT, S>(c, IntC<LI + 1>{});
+      request_layer_history<AI, NT>(c, IntC<LI + 1>{});
     else if constexpr (HEADK > 1)
     {
       if (c.warp == 0) // the head accumulator's own ring (A2 family: head{kernel_size: 16}, model.cpp:397-400)
-        hist_load<HP, HL, HRMASK, W>(c.buf, c.state + S * HROFF, c.tabs0, c.bar, c.lane);
+        hist_load<P, HL, HRMASK, W>(c.buf, c.state + HROFF, c.tabs0, c.bar, c.lane);
     }
     else if constexpr (NEXT_AI >= 0)
-      request_layer_history<NEXT_AI, NT, S>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
+      request_layer_history<NEXT_AI, NT>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
 
     // ---- phase 2: h_{l+1} = h_l + p + P a  (model.cpp:243,376)
-    V hn[C];
+    float hn[C];
 #pragma unroll
     for (int pl = 0; pl < P; pl++)
     {
-      V own[4];
+      float own[4];
       load_plane<W>(col0, pl, 0, own);
 #pragma unroll
       for (int i = 0; i < 4; i++)
-        hn[4 * pl + i] = vaddc(own[i], spec::w(w_pb + 4 * pl + i));
+        hn[4 * pl + i] = own[i] + spec::w(w_pb + 4 * pl + i);
     }
 #pragma unroll
     for (int i = 0; i < C; i++)
 #pragma unroll
       for (int o = 0; o < C; o++)
-        hn[o] = vfma(acc[i], spec::w(w_p + i * C + o), hn[o]);
+        hn[o] = fmaf(spec::w(w_p + i * C + o), acc[i], hn[o]);
     if constexpr (!last)
     {
 #pragma unroll
       for (int pl = 0; pl < P; pl++)
       {
-        const V q[4] = {hn[4 * pl], hn[4 * pl + 1], hn[4 * pl + 2], hn[4 * pl + 3]};
+        const float q[4] = {hn[4 * pl], hn[4 * pl + 1], hn[4 * pl + 2], hn[4 * pl + 3]};
         store_plane<W>(col0, pl, q);
       }
     }
@@ -580,7 +457,7 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A
 #pragma unroll
     for (int pl = 0; pl < P; pl++)
     {
-      const V q[4] = {head[4 * pl], head[4 * pl + 1], head[4 * pl + 2], head[4 * pl + 3]};
+      const float q[4] = {head[4 * pl], head[4 * pl + 1], head[4 * pl + 2], head[4 * pl + 3]};
       store_plane<W>(col0, pl, q);
     }
     fence_async_smem();
@@ -588,10 +465,10 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A
     mbar_wait(c.bar, c.phase);
     c.phase ^= 1u;
     if (c.warp == 0)
-      hist_store<HP, HL, A.head_ring_mask, W>(c.buf, c.state + S * A.head_ring_off, c.tabs0, c.tv, c.lane);
+      hist_store<P, HL, A.head_ring_mask, W>(c.buf, c.state + A.head_ring_off, c.tabs0, c.tv, c.lane);
 #pragma unroll
     for (int ho = 0; ho < HOUT; ho++)
-      vsplat(headout[ho], spec::w(A.head_off + HK * C * HOUT + ho)); // bias first, like the fused kernel
+      headout[ho] = spec::w(A.head_off + HK * C * HOUT + ho); // bias first, like the fused kernel
 #pragma unroll
     for (int k = 0; k < HK; k++)
     {
@@ -599,93 +476,43 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const V (&hin)[spec::A
 #pragma unroll
       for (int pl = 0; pl < P; pl++)
       {
-        V x[4];
+        float x[4];
         load_plane<W>(col0, pl, off, x);
 #pragma unroll
         for (int i = 0; i < 4; i++)
 #pragma unroll
           for (int ho = 0; ho < HOUT; ho++)
-            headout[ho] = vfma(x[i], spec::w(A.head_off + (k * C + 4 * pl + i) * HOUT + ho), headout[ho]);
+            headout[ho] = fmaf(spec::w(A.head_off + (k * C + 4 * pl + i) * HOUT + ho), x[i], headout[ho]);
       }
     }
-    if (c.warp == 0 && c.lane < HP)
+    if (c.warp == 0 && c.lane < P)
       bulk_wait_all();
     __syncthreads(); // every read of the accumulator columns is done
     if constexpr (NEXT_AI >= 0)
-      request_layer_history<NEXT_AI, NT, S>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
+      request_layer_history<NEXT_AI, NT>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
     return;
   }
 
   // ---- head rechannel (kernel size 1; model.cpp:548): headout = H head (+ g)
 #pragma unroll
   for (int ho = 0; ho < HOUT; ho++)
-    vsplat(headout[ho], 0.0f);
+    headout[ho] = 0.0f;
 #pragma unroll
   for (int i = 0; i < C; i++)
 #pragma unroll
     for (int ho = 0; ho < HOUT; ho++)
-      headout[ho] = vfma(head[i], spec::w(A.head_off + i * HOUT + ho), headout[ho]);
+      headout[ho] = fmaf(spec::w(A.head_off + i * HOUT + ho), head[i], headout[ho]);
 #pragma unroll
   for (int ho = 0; ho < HOUT; ho++)
-    headout[ho] = vaddc(headout[ho], spec::w(A.head_off + C * HOUT + ho)); // bias (zero when the head has none)
+    headout[ho] += spec::w(A.head_off + C * HOUT + ho); // bias (zero when the head has none)
 }
 
-template <int NT>
-__device__ __forceinline__ void pair_rings_to_scratch(const float* ra, const float* rb, float* sc)
+template <int NT, int MINB>
+__device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
 {
-  static_for<0, spec::NL>([&](auto li_c) {
-    constexpr int LI = decltype(li_c)::value;
-    constexpr spec::Layer Ld = spec::L[LI];
-    constexpr int R = Ld.ring_mask + 1;
-    constexpr int C = spec::layer_channels(LI);
-    const float4* a4 = reinterpret_cast<const float4*>(ra + Ld.ring_off);
-    const float4* b4 = reinterpret_cast<const float4*>(rb + Ld.ring_off);
-    float4* s4 = reinterpret_cast<float4*>(sc + 2 * Ld.ring_off);
-    for (int idx = threadIdx.x; idx < (C / 4) * R; idx += NT)
-    {
-      const int pl = idx / R, col = idx - pl * R;
-      const float4 a = __ldcg(a4 + idx), b = __ldcg(b4 + idx);
-      __stcg(s4 + (2 * pl) * R + col, make_float4(a.x, b.x, a.y, b.y));
-      __stcg(s4 + (2 * pl + 1) * R + col, make_float4(a.z, b.z, a.w, b.w));
-    }
-  });
-}
-template <int NT>
-__device__ __forceinline__ void pair_scratch_to_rings(const float* sc, float* ra, float* rb, const bool live_b)
-{
-  static_for<0, spec::NL>([&](auto li_c) {
-    constexpr int LI = decltype(li_c)::value;
-    constexpr spec::Layer Ld = spec::L[LI];
-    constexpr int R = Ld.ring_mask + 1;
-    constexpr int C = spec::layer_channels(LI);
-    float4* a4 = reinterpret_cast<float4*>(ra + Ld.ring_off);
-    float4* b4 = reinterpret_cast<float4*>(rb + Ld.ring_off);
-    const float4* s4 = reinterpret_cast<const float4*>(sc + 2 * Ld.ring_off);
-    for (int idx = threadIdx.x; idx < (C / 4) * R; idx += NT)
-    {
-      const int pl = idx / R, col = idx - pl * R;
-      const float4 q0 = __ldcg(s4 + (2 * pl) * R + col), q1 = __ldcg(s4 + (2 * pl + 1) * R + col);
-      __stcg(a4 + idx, make_float4(q0.x, q0.z, q1.x, q1.z));
-      if (live_b)
-        __stcg(b4 + idx, make_float4(q0.y, q0.w, q1.y, q1.w));
-    }
-  });
-}
-// generic-proxy global accesses <-> the bulk (async-proxy) copies on the scratch
-__device__ __forceinline__ void fence_async_all()
-{
-  asm volatile("fence.proxy.async;" ::: "memory");
-}
-
-template <int NT, int S, int MINB>
-__device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
-{
-  static_assert(S == 1 || (spec::A[0].head_kernel == 1 && spec::A[spec::NA - 1].head_kernel == 1),
-                "the stream-pair variant does not convert head rings");
-  constexpr int T = NT; // one frame per thread (of one stream, or of a pair of streams)
+  constexpr int T = NT; // one frame per thread
   static_assert(spec::NA == 1 || spec::NA == 2, "one or two layer arrays");
-  static_assert(S == 1 || S == 2, "one stream per thread, or a packed pair of streams");
-  extern __shared__ float4 spec_smem[]; // [(sub-)planes][W] float4
+  extern __shared__ float4 spec_smem[]; // [planes][W] float4
   __shared__ u64 bar;
   const int tid = threadIdx.x;
   TileCtx c;
@@ -701,96 +528,53 @@ __device__ __forceinline__ void wavenet_spec_body(const SpecParams& p)
   }
   __syncthreads();
 
-  typedef typename FrameVec<S>::type V;
-  const int n_units = (S == 1) ? p.batch : (p.batch + 1) / 2; // streams, or pairs of streams
-  for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x)
+  const int batch = p.batch;
+  for (int s = blockIdx.x; s < batch; s += gridDim.x)
   {
-    const int sa = S * unit, sb = min(sa + 1, p.batch - 1);
-    const bool live_b = (S == 2) && (sa + 1 < p.batch); // an odd batch leaves the last pair's second half idle
-    const bool table = (S == 1) && p.slots != nullptr;
-    float* const state_a = p.state + (size_t)(table ? p.slots[sa].stream : sa) * p.state_stride;
-    float* const state_b = p.state + (size_t)sb * p.state_stride;
-    const u32 clock_a = table ? p.slots[sa].clock : p.t_base;
-    const int n_a = table ? p.slots[sa].frames : p.n_frames; // the stream's own frames (CTA-uniform: one stream)
-    const float* xin_a = p.in + (size_t)sa * p.in_stride;
-    const float* xin_b = p.in + (size_t)sb * p.in_stride;
-    float* yout_a = p.out + (size_t)sa * p.out_stride;
-    float* yout_b = p.out + (size_t)sb * p.out_stride;
-    if constexpr (S == 1)
-      c.state = state_a;
-    else
+    const bool table = p.slots != nullptr;
+    float* const state = p.state + (size_t)(table ? p.slots[s].stream : s) * p.state_stride;
+    const u32 clock = table ? p.slots[s].clock : p.t_base;
+    const int n = table ? p.slots[s].frames : p.n_frames; // the stream's own frames (CTA-uniform: one stream)
+    const float* xin = p.in + (size_t)s * p.in_stride;
+    float* yout = p.out + (size_t)s * p.out_stride;
+    c.state = state;
+    for (int t0 = 0; t0 < n; t0 += T)
     {
-      c.state = p.scratch + (size_t)blockIdx.x * p.scratch_stride;
-      pair_rings_to_scratch<NT>(state_a, state_b, c.state);
-      fence_async_all(); // my scratch stores (generic proxy) -> the bulk loads below
-      __syncthreads();
-    }
-    for (int t0 = 0; t0 < n_a; t0 += T)
-    {
-      c.tv = min(T, n_a - t0);
-      c.tabs0 = clock_a + (u32)t0;
-      request_layer_history<0, NT, S>(c, IntC<spec::A[0].layer0>{});
-      V x[1];
-      {
-        const float xa = (tid < c.tv) ? __ldg(xin_a + t0 + tid) : 0.0f;
-        if constexpr (S == 1)
-          x[0] = xa;
-        else
-          x[0] = pack2(xa, (live_b && tid < c.tv) ? __ldg(xin_b + t0 + tid) : 0.0f);
-      }
-      const V cond = x[0]; // no condition_dsp: condition == input (model.cpp:781)
-      V y;
+      c.tv = min(T, n - t0);
+      c.tabs0 = clock + (u32)t0;
+      request_layer_history<0, NT>(c, IntC<spec::A[0].layer0>{});
+      float x[1];
+      x[0] = (tid < c.tv) ? __ldg(xin + t0 + tid) : 0.0f;
+      const float cond = x[0]; // no condition_dsp: condition == input (model.cpp:781)
+      float y;
       constexpr int C0 = spec::A[0].C;
-      V head0[C0], hout0[C0], ho0[spec::A[0].HOUT];
+      float head0[C0], hout0[C0], ho0[spec::A[0].HOUT];
 #pragma unroll
       for (int o = 0; o < C0; o++)
-        vsplat(head0[o], 0.0f); // model.cpp:469
+        head0[o] = 0.0f; // model.cpp:469
       if constexpr (spec::NA == 1)
       {
-        array_forward<0, -1, NT, S, V>(c, x, cond, head0, hout0, ho0);
+        array_forward<0, -1, NT>(c, x, cond, head0, hout0, ho0);
         y = ho0[0];
       }
       else
       {
-        array_forward<0, spec::NA - 1, NT, S, V>(c, x, cond, head0, hout0, ho0);
+        array_forward<0, spec::NA - 1, NT>(c, x, cond, head0, hout0, ho0);
         // second array: layer input = the previous array's layer output, head accumulator starts from the previous
         // array's head output (model.cpp:846-848, :473-486)
         constexpr int AI1 = spec::NA - 1;
         constexpr int C1 = spec::A[AI1].C;
-        V head1[C1], hout1[C1], ho1[spec::A[AI1].HOUT];
+        float head1[C1], hout1[C1], ho1[spec::A[AI1].HOUT];
 #pragma unroll
         for (int o = 0; o < C1; o++)
           head1[o] = ho0[o];
-        array_forward<AI1, -1, NT, S, V>(c, hout0, cond, head1, hout1, ho1);
+        array_forward<AI1, -1, NT>(c, hout0, cond, head1, hout1, ho1);
         y = ho1[0];
       }
       // model.cpp:888-897
-      if constexpr (S == 1)
-      {
-        if (tid < c.tv)
-          yout_a[t0 + tid] = spec::head_scale * y;
-      }
-      else
-      {
-        float ya, yb;
-        unpack2(y, ya, yb);
-        if (tid < c.tv)
-        {
-          yout_a[t0 + tid] = spec::head_scale * ya;
-          if (live_b)
-            yout_b[t0 + tid] = spec::head_scale * yb;
-        }
-      }
+      if (tid < c.tv)
+        yout[t0 + tid] = spec::head_scale * y;
       // (no barrier here: the last layer's B1 already fenced every tap read before anything of the next tile is written)
-    }
-    if constexpr (S == 2)
-    {
-      // every bulk store of the call has completed (each issuing lane waited before the last B1); make them visible to
-      // the generic loads of the conversion, then hand the rings back in the library's layout
-      fence_async_all();
-      __syncthreads();
-      pair_scratch_to_rings<NT>(c.state, state_a, state_b, live_b);
-      __syncthreads(); // the scratch is rewritten for the next pair
     }
   }
 }
@@ -1026,7 +810,7 @@ __device__ __forceinline__ void array_forward_short(float4* tile, float* state, 
 }
 
 template <int NT, int FQ>
-__device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
+__device__ __forceinline__ void wavenet_spec_short_body(const JitParams& p)
 {
   constexpr int Q = NT / FQ; // streams per CTA
   static_assert(Q * FQ == NT && (FQ % 32) == 0, "whole warps per stream");
@@ -1077,9 +861,6 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
 #ifndef NAMB200_SPEC_NT
 #define NAMB200_SPEC_NT 512
 #endif
-#ifndef NAMB200_SPEC_S
-#define NAMB200_SPEC_S 1
-#endif
 #ifndef NAMB200_SPEC_MINB
 #define NAMB200_SPEC_MINB 2
 #endif
@@ -1088,9 +869,9 @@ __device__ __forceinline__ void wavenet_spec_short_body(const SpecParams& p)
 // variant in the first, the 128- / 256-frame variants in the second, NAMB200_SPEC_ONLY_EXTRA_SHORT)
 #ifndef NAMB200_SPEC_ONLY_EXTRA_SHORT
 extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_NT, NAMB200_SPEC_MINB)
-  wavenet_spec_kernel(const __grid_constant__ namb200_spec::SpecParams p)
+  wavenet_spec_kernel(const __grid_constant__ namb200::JitParams p)
 {
-  namb200_spec::wavenet_spec_body<NAMB200_SPEC_NT, NAMB200_SPEC_S, NAMB200_SPEC_MINB>(p);
+  namb200_spec::wavenet_spec_body<NAMB200_SPEC_NT, NAMB200_SPEC_MINB>(p);
 }
 #endif
 #if defined(NAMB200_SPEC_SHORT_FQ) && !defined(NAMB200_SPEC_ONLY_EXTRA_SHORT)
@@ -1099,7 +880,7 @@ extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_NT, NAMB200_SPEC_MINB)
 #define NAMB200_SPEC_SHORT_NT NAMB200_SPEC_NT
 #endif
 extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_SHORT_NT, 2)
-  wavenet_spec_short_kernel(const __grid_constant__ namb200_spec::SpecParams p)
+  wavenet_spec_short_kernel(const __grid_constant__ namb200::JitParams p)
 {
   namb200_spec::wavenet_spec_short_body<NAMB200_SPEC_SHORT_NT, NAMB200_SPEC_SHORT_FQ>(p);
 }
@@ -1107,14 +888,14 @@ extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_SHORT_NT, 2)
 // the same for calls of up to 128 / 256 frames (hosts with larger audio buffers): NT / 128 and NT / 256 streams per CTA
 #ifdef NAMB200_SPEC_SHORT128_NT
 extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_SHORT128_NT, 2)
-  wavenet_spec_short128_kernel(const __grid_constant__ namb200_spec::SpecParams p)
+  wavenet_spec_short128_kernel(const __grid_constant__ namb200::JitParams p)
 {
   namb200_spec::wavenet_spec_short_body<NAMB200_SPEC_SHORT128_NT, 128>(p);
 }
 #endif
 #ifdef NAMB200_SPEC_SHORT256_NT
 extern "C" __global__ void __launch_bounds__(NAMB200_SPEC_SHORT256_NT, 2)
-  wavenet_spec_short256_kernel(const __grid_constant__ namb200_spec::SpecParams p)
+  wavenet_spec_short256_kernel(const __grid_constant__ namb200::JitParams p)
 {
   namb200_spec::wavenet_spec_short_body<NAMB200_SPEC_SHORT256_NT, 256>(p);
 }

@@ -38,9 +38,9 @@ int main(int argc, char** argv)
   for (size_t i = 0; i < h.size(); i++)
     h[i] = 0.3f * sinf(0.01f * (float)(i % 100003));
   CK(cudaMemcpy(in, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
-  namb200_lat::LatParams p{state, spec::state_floats, in, out, n, n, batch, n, 0u, nullptr, 0u};
+  namb200::LatParams p{{state, spec::state_floats, in, out, n, n, batch, n, 0u, nullptr}, nullptr, 0u};
   {
-    // correctness: the same calls through the throughput kernel (wavenet_spec.cuh, S = 1) on a second copy of the state
+    // correctness: the same calls through the throughput kernel (wavenet_spec.cuh) on a second copy of the state
     float *state2, *out2;
     CK(cudaMalloc(&state2, (size_t)batch * spec::state_floats * 4));
     CK(cudaMemset(state2, 0, (size_t)batch * spec::state_floats * 4));
@@ -50,7 +50,7 @@ int main(int argc, char** argv)
       pmax = spec::A[a].C / 4 > pmax ? spec::A[a].C / 4 : pmax;
     const size_t smem2 = (size_t)pmax * (spec::LS + NAMB200_SPEC_NT) * 16;
     CK(cudaFuncSetAttribute(wavenet_spec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    namb200_spec::SpecParams q{state2, spec::state_floats, in, out2, n, n, batch, n, 0u, nullptr, 0};
+    namb200::JitParams q{state2, spec::state_floats, in, out2, n, n, batch, n, 0u, nullptr};
     std::vector<float> a(h.size()), b(h.size());
     double worst = 0;
     for (int call = 0; call < 40; call++)

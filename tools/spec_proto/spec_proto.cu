@@ -24,11 +24,11 @@
 int main(int argc, char** argv)
 {
   const int batch = argc > 1 ? atoi(argv[1]) : 4096, n = argc > 2 ? atoi(argv[2]) : 4096, reps = argc > 3 ? atoi(argv[3]) : 5;
-  constexpr int NT = NAMB200_SPEC_NT, S = NAMB200_SPEC_S, MINB = NAMB200_SPEC_MINB;
+  constexpr int NT = NAMB200_SPEC_NT, MINB = NAMB200_SPEC_MINB;
   int pmax = 0;
   for (int a = 0; a < spec::NA; a++)
     pmax = spec::A[a].C / 4 > pmax ? spec::A[a].C / 4 : pmax;
-  const size_t smem = (size_t)pmax * S * (spec::LS + NT) * 16; // S = 2: twice the (sub-)planes
+  const size_t smem = (size_t)pmax * (spec::LS + NT) * 16;
   CK(cudaFuncSetAttribute(wavenet_spec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, wavenet_spec_kernel, NT, smem));
@@ -46,10 +46,7 @@ int main(int argc, char** argv)
   for (size_t i = 0; i < h.size(); i++)
     h[i] = 0.3f * sinf(0.01f * (float)(i % 100003));
   CK(cudaMemcpy(in, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
-  float* scratch = nullptr;
-  if (S == 2)
-    CK(cudaMalloc(&scratch, (size_t)grid * 2 * spec::state_floats * 4));
-  namb200_spec::SpecParams p{state, spec::state_floats, in, out, n, n, batch, n, 0u, scratch, 2 * spec::state_floats};
+  namb200::JitParams p{state, spec::state_floats, in, out, n, n, batch, n, 0u, nullptr};
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
@@ -71,8 +68,8 @@ int main(int argc, char** argv)
   double cs = 0;
   for (size_t i = 0; i < h.size(); i += 997)
     cs += h[i];
-  printf("{\"test\": \"spec_proto\", \"NT\": %d, \"S\": %d, \"minb\": %d, \"regs\": %d, \"ctas_per_sm\": %d, \"smem\": %zu, \"batch\": %d, "
+  printf("{\"test\": \"spec_proto\", \"NT\": %d, \"minb\": %d, \"regs\": %d, \"ctas_per_sm\": %d, \"smem\": %zu, \"batch\": %d, "
          "\"n\": %d, \"ms\": %.3f, \"msamples_per_s\": %.1f, \"checksum\": %.6g}\n",
-         NT, S, MINB, fa.numRegs, occ, smem, batch, n, best, (double)batch * n / best / 1e3, cs);
+         NT, MINB, fa.numRegs, occ, smem, batch, n, best, (double)batch * n / best / 1e3, cs);
   return 0;
 }
