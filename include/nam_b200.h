@@ -169,37 +169,55 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
 /* ---- model banks: one handle, streams of different captures of one architecture ----------------------------------------
  * A bank is a handle created from K >= 1 .nam documents of one shape; each of its max_batch streams is bound to one of the
  * K models, and every process call runs each listed stream with its own model's weights, in the launches an ordinary
- * handle's call of that batch takes.  Which documents can share a bank:
- *   - every one served by the fused WaveNet kernel family (wavenet.nam, a1_standard, A2-Lite and A2-Full shapes): not the
- *     general kernel (gated, FiLM, ...), ConvNet, LSTM, Linear, SlimmableContainer files or slimmable WaveNets;
- *   - models 1.. equal to model 0 in everything but their weights: layer arrays, channels, kernel sizes, dilations,
- *     activations and their parameters, hence the packed kernel layout and blob length; the config object apart from its
- *     unused head_scale field (head_scale is the last weight, so it is per model); the expected sample rate.
- *   Refusals (NAM_B200_ERR_UNSUPPORTED for a model outside the family, NAM_B200_ERR_MODEL for a mismatch) name the first
- *   offending model index and the field.  jit = 1 is refused (a model-specialised kernel compiles one model's weights into
- *   its code); jit = 0 or 3 silently keeps the precompiled kernels, and nam_b200_jit_note says so.  kernel_geometry 4 (the
- *   general kernel) is refused.  A bank of one document is exactly nam_b200_create_from_json / _from_file, JIT included.
- * All streams start bound to model 0.  Every call of this header works on a bank:
+ * handle's call of that batch takes.  Which documents can share a bank -- model 0 chooses one of two families:
+ *   - WaveNets served by the fused kernel family (wavenet.nam, a1_standard, A2-Lite and A2-Full shapes): not the general
+ *     kernel (gated, FiLM, ...), SlimmableContainer files or slimmable WaveNets.  Models 1.. equal model 0 in everything
+ *     but their weights: layer arrays, channels, kernel sizes, dilations, activations and their parameters, hence the
+ *     packed kernel layout and blob length; the config object apart from its unused head_scale field (head_scale is the
+ *     last weight, so it is per model); the expected sample rate.
+ *   - LSTMs an ordinary handle serves (a model it would refuse is refused with its reason).  Models 1.. equal model 0 in
+ *     the expected sample rate (hence the prewarm length), in_channels and out_channels, num_layers, input_size,
+ *     hidden_size and the config object; their weights, trained h0 / c0 and head are per model.
+ *   ConvNet, Linear and mixed families are refused.  Refusals (NAM_B200_ERR_UNSUPPORTED for a model outside the family,
+ *   NAM_B200_ERR_MODEL for a mismatch) name the first offending model index and the field.  jit = 1 is refused (a
+ *   model-specialised kernel compiles one model's weights into its code); jit = 0 or 3 silently keeps the precompiled
+ *   kernels, and nam_b200_jit_note says so.  kernel_geometry 4 (the general kernel) is refused.  A bank of one document is
+ *   exactly nam_b200_create_from_json / _from_file, JIT included.
+ * All streams start bound to model 0.  Every call of this header works on a bank, each stream exactly (bit for bit) as the
+ * same stream of an ordinary jit = 2 handle of its model:
  *   - process calls (nam_b200_process_f32 and _device, process_streams*, the ragged calls, the planar DSP::process on stream
  *     0, the pipelined host path): each stream runs its own model;
- *   - nam_b200_reset / nam_b200_prewarm: every stream ends in the (prewarmed) state of its own model;
- *   - reset_streams: as nam_b200_assign_streams to each stream's current model;
+ *   - nam_b200_reset: a WaveNet stream ends in the prewarmed fresh state of its own model.  An LSTM keeps h, c across
+ *     Reset: each stream is prewarmed in place with its own model (from h0 / c0 the first time, since creation writes every
+ *     stream's h0 / c0);
+ *   - nam_b200_prewarm: every stream is prewarmed from its current state with its own model;
+ *   - reset_streams: a WaveNet stream, and an LSTM stream with fresh = 1, takes its current model's fresh state; an LSTM
+ *     stream with fresh = 0 is prewarmed in place with its model;
  *   - copy_streams: the destination takes the source's model along with its state;
  *   - export_streams: a record carries the fingerprint of its stream's model;
  *   - import_streams: accepts a record of any model of the bank and binds the stream to it (with duplicate documents the
  *     lowest such index); a fingerprint outside the bank is refused, naming it.  A session therefore moves between a bank
- *     and an ordinary handle of its model in either direction.
- * Device memory: the K blobs (a1_standard: ~14k floats each) and K output scales, plus K "model rows" of per-stream state
- * (a1_standard: 196 KB each) that hold every model's freshly reset state: reset prewarms them together and copies each
- * stream its model's row; reset_streams and assign_streams copy them again (one launch whatever the mix). */
+ *     and an ordinary handle of its model in either direction;
+ *   - nam_b200_set_fast_tanh: as on an ordinary handle (an LSTM bank rebuilds its model rows in the new regime before the
+ *     next fresh-state copy).
+ * Device memory: the K blobs (a1_standard: ~14k floats each; lstm.nam: 64 floats each) and, for WaveNets,
+ * K output scales, plus K "model rows" of state_stride floats each (a1_standard: 196 KB each; lstm.nam: 8 floats) that
+ * hold every model's freshly reset state (an LSTM's: h0 / c0 plus the prewarm): reset prewarms them together -- an LSTM
+ * bank in the same launches as its streams -- and reset_streams and assign_streams copy them (one launch whatever the mix).
+ * Cost of mixing: an LSTM kernel's CTA holds several streams (lane groups: 128 / G of them; thread per stream: 64); the
+ * lane-group kernel keeps one weight copy per distinct model of a CTA where they fit and makes another pass where they do
+ * not, the thread-per-stream kernel makes one pass per distinct model (up to 64 with round-robin binding).  Keep a model's
+ * streams in adjacent slots. */
 int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const nam_b200_options* opts, nam_b200_model** out);
 int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out);
 /* K of a bank; 1 for every other handle (so model index 0 is valid on every handle). */
 int nam_b200_bank_size(const nam_b200_model* m);
 /* Bind streams[i] to model models[i] and put it in the state of a freshly reset handle of that model (the reset_streams
- * contract, per model); every other stream is untouched.  Checked on the host like the other stream lists (distinct
- * streams in [0, max_batch), model indices in [0, bank_size), after reset); a refusal names the entry.  On an ordinary
- * handle, models all 0 is nam_b200_reset_streams. */
+ * contract, per model: for an LSTM, reset_streams with fresh = 1 on an ordinary handle of that model); every other stream
+ * is untouched.  Checked on the host like the other stream lists (distinct streams in [0, max_batch), model indices in
+ * [0, bank_size), after reset); a refusal names the entry.  On an ordinary handle (K = 1), models all 0 is
+ * nam_b200_reset_streams with fresh = 0 -- for an LSTM that keeps the running state and prewarms on top, unlike a bank of
+ * K >= 2, which restarts the stream from its new model's h0 / c0. */
 int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, const int32_t* models);
 /* out[i] = the model streams[i] is bound to. */
 int nam_b200_stream_models(const nam_b200_model* m, const int32_t* streams, int n, int32_t* out);

@@ -22,7 +22,7 @@ struct StreamRef
   union
   {
     int alt; // Linear: the stream's history is in the alternate buffer of the double buffer
-    int model; // fused WaveNet family: the model of a bank (nam_b200_create_bank_*) this position runs; 0 otherwise
+    int model; // fused WaveNet family and LSTM: the model of a bank (nam_b200_create_bank_*) this position runs; 0 otherwise
   };
   // process calls: frames this position runs, in [0, n_frames] of the launch (n_frames is the buffers' frame pitch).  A
   // position stops at its own count: frames past it are neither read nor written, and a stream with 0 keeps its state.

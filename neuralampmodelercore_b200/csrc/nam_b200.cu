@@ -95,6 +95,10 @@ struct LstmKernelParams
   int in_ch, out_ch;
   // slot table (nullptr: position b is state row b): position b uses state row slots[b].stream; in / out stay by position
   const StreamRef* slots;
+  // model bank (the BANK instantiations; they always get a table): position b runs model slots[b].model, whose blob starts
+  // at weights + model * weight_stride.  bank_copies: the model copies lstm_group_kernel's shared memory holds.
+  long weight_stride;
+  int bank_copies;
 };
 
 constexpr int kLstmThreads = 64; // streams per CTA
@@ -110,6 +114,11 @@ __device__ __forceinline__ float lstm_tanh(float x, int fast)
   return fast ? act_fast_tanh(x) : tanhf(x);
 }
 
+// BANK (model banks): the weights of one model fill shared memory, so the CTA runs one pass of the chunk loop per distinct
+// model among its positions, that model's blob staged for the pass; a position outside the pass runs 0 frames in it (its
+// state stays as it is, it writes no output).  Positions of one model in adjacent slots keep a CTA at one pass; round-robin
+// binding of 64 or more models costs up to 64.  Each stream's arithmetic is the ordinary instantiation's.
+template <bool BANK = false>
 __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelParams p)
 {
   extern __shared__ float smem[];
@@ -121,8 +130,9 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
   float* sio = sgate + 4 * H * kLstmThreads; // [kLstmThreads][kLstmChunk+1] in, then same for out
   float* sout = sio + kLstmThreads * (kLstmChunk + 1);
 
-  for (int i = tid; i < p.n_weight_floats; i += kLstmThreads)
-    sw[i] = __ldg(p.weights + i);
+  if constexpr (!BANK)
+    for (int i = tid; i < p.n_weight_floats; i += kLstmThreads)
+      sw[i] = __ldg(p.weights + i);
   const int stream = blockIdx.x * kLstmThreads + tid;
   const bool active = stream < p.batch;
   const size_t row = p.slots ? (size_t)p.slots[active ? stream : 0].stream : (size_t)stream;
@@ -130,107 +140,132 @@ __global__ void __launch_bounds__(kLstmThreads) lstm_kernel(const LstmKernelPara
   if (active)
     for (int i = 0; i < n_state; i++)
       sstate[i * kLstmThreads + tid] = p.state[row * p.state_stride + i];
+  const int stream0 = blockIdx.x * kLstmThreads;
+  // BANK: s_model[s] = the model of position s (-1 beyond the batch), s_first[s] = the first position of that model
+  __shared__ int s_model[BANK ? kLstmThreads : 1], s_first[BANK ? kLstmThreads : 1];
+  if constexpr (BANK)
+  {
+    s_model[tid] = active ? p.slots[stream].model : -1;
+    __syncthreads();
+    int first = tid;
+    for (int s = tid - 1; s >= 0; s--)
+      first = s_model[s] == s_model[tid] ? s : first;
+    s_first[tid] = s_model[tid] < 0 ? -1 : first;
+  }
   __syncthreads();
 
-  const int stream0 = blockIdx.x * kLstmThreads;
-  // frames of the CTA's position s (slot table: the stream's own count; 0 beyond the batch); the chunk loop holds
-  // barriers, so it runs to the CTA's longest stream
-  auto frames_of = [&](int s) -> int {
-    const int b = stream0 + s;
-    return b >= p.batch ? 0 : p.slots ? p.slots[b].frames : p.n_frames;
-  };
-  int n_cta = 0;
-  for (int s = 0; s < kLstmThreads; s++)
-    n_cta = max(n_cta, frames_of(s));
-  const int n_me = frames_of(tid);
-  for (int t0 = 0; t0 < n_cta; t0 += kLstmChunk)
+  // one pass per distinct model, led by its first position (an ordinary CTA: one pass over every position)
+  for (int lead = 0; lead < (BANK ? kLstmThreads : 1); lead++)
   {
-    // coalesced load of the [streams x chunk] input tile
-    for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
+    if constexpr (BANK)
     {
-      const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
-      float v = 0.0f;
-      if (t0 + f < frames_of(s))
-        v = __ldg(p.in + (size_t)(stream0 + s) * p.in_stride + t0 + f);
-      sio[s * (kLstmChunk + 1) + f] = v;
+      if (s_first[lead] != lead) // (uniform: shared)
+        continue;
+      const float* src = p.weights + (size_t)s_model[lead] * p.weight_stride;
+      for (int i = tid; i < p.n_weight_floats; i += kLstmThreads)
+        sw[i] = __ldg(src + i); // (the previous pass's last barrier ordered its reads before these writes)
     }
-    __syncthreads();
-    const int tc = min(kLstmChunk, n_me - t0); // this thread's frames in the chunk (<= 0: its stream has ended)
-    if (active)
+    // frames of the CTA's position s in this pass (slot table: the stream's own count; 0 beyond the batch and, in a bank, for
+    // another model's position); the chunk loop holds barriers, so it runs to the pass's longest stream
+    auto frames_of = [&](int s) -> int {
+      const int b = stream0 + s;
+      if (BANK && s_model[s] != s_model[lead])
+        return 0;
+      return b >= p.batch ? 0 : p.slots ? p.slots[b].frames : p.n_frames;
+    };
+    int n_cta = 0;
+    for (int s = 0; s < kLstmThreads; s++)
+      n_cta = max(n_cta, frames_of(s));
+    const int n_me = frames_of(tid);
+    for (int t0 = 0; t0 < n_cta; t0 += kLstmChunk)
     {
-      const bool multi = p.in_ch > 1 || p.out_ch > 1;
-      const float* __restrict__ gin = p.in + (size_t)stream * p.in_stride + t0;
-      float* __restrict__ gout = p.out + (size_t)stream * p.out_stride + t0;
-      for (int f = 0; f < tc; f++)
+      // coalesced load of the [streams x chunk] input tile
+      for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
       {
-        float x_scalar = sio[tid * (kLstmChunk + 1) + f];
-        const float* w = sw;
-        for (int l = 0; l < p.num_layers; l++)
-        {
-          const int I = (l == 0) ? p.input_size : H;
-          const int W = I + H;
-          float* hs = sstate + (l * 2) * H * kLstmThreads;
-          float* cs = hs + H * kLstmThreads;
-          const float* xprev = (l == 0) ? nullptr : sstate + ((l - 1) * 2) * H * kLstmThreads;
-          const float* b = w + 4 * H * W;
-          // ifgo = W [x ; h] + b   (lstm.cpp:36-40); rows ordered i, f, g, o
-          for (int r = 0; r < 4 * H; r++)
-          {
-            const float* wr = w + r * W;
-            float acc = 0.0f;
-            if (l == 0 && !multi)
-              acc = fmaf(wr[0], x_scalar, acc); // input_size == 1
-            else if (l == 0)
-              for (int j = 0; j < I; j++)
-                acc = fmaf(wr[j], __ldg(gin + (size_t)j * p.n_frames + f), acc);
-            else
-              for (int j = 0; j < I; j++)
-                acc = fmaf(wr[j], xprev[j * kLstmThreads + tid], acc);
-            for (int j = 0; j < H; j++)
-              acc = fmaf(wr[I + j], hs[j * kLstmThreads + tid], acc);
-            sgate[r * kLstmThreads + tid] = acc + b[r];
-          }
-          for (int i = 0; i < H; i++)
-          {
-            const float gi = sgate[(i)*kLstmThreads + tid];
-            const float gf = sgate[(H + i) * kLstmThreads + tid];
-            const float gg = sgate[(2 * H + i) * kLstmThreads + tid];
-            const float go = sgate[(3 * H + i) * kLstmThreads + tid];
-            const float c = lstm_sigmoid(gf, p.fast_tanh) * cs[i * kLstmThreads + tid]
-                            + lstm_sigmoid(gi, p.fast_tanh) * lstm_tanh(gg, p.fast_tanh); // lstm.cpp:50-53,61-63
-            cs[i * kLstmThreads + tid] = c;
-            hs[i * kLstmThreads + tid] = lstm_sigmoid(go, p.fast_tanh) * lstm_tanh(c, p.fast_tanh); // :55-57,65-66
-          }
-          w = b + 4 * H;
-        }
-        // head (lstm.cpp:164-167)
-        const float* hl = sstate + ((p.num_layers - 1) * 2) * H * kLstmThreads;
-        if (multi)
-        {
-          // head: (out_channels x H) row-major, then the bias vector (lstm.cpp:79-97)
-          for (int oc = 0; oc < p.out_ch; oc++)
-          {
-            float y = 0.0f;
-            for (int j = 0; j < H; j++)
-              y = fmaf(w[oc * H + j], hl[j * kLstmThreads + tid], y);
-            gout[(size_t)oc * p.n_frames + f] = y + w[p.out_ch * H + oc];
-          }
-          continue;
-        }
-        float y = 0.0f;
-        for (int j = 0; j < H; j++)
-          y = fmaf(w[j], hl[j * kLstmThreads + tid], y);
-        sout[tid * (kLstmChunk + 1) + f] = y + w[H];
+        const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
+        float v = 0.0f;
+        if (t0 + f < frames_of(s))
+          v = __ldg(p.in + (size_t)(stream0 + s) * p.in_stride + t0 + f);
+        sio[s * (kLstmChunk + 1) + f] = v;
       }
+      __syncthreads();
+      const int tc = min(kLstmChunk, n_me - t0); // this thread's frames in the chunk (<= 0: its stream has ended)
+      if (active)
+      {
+        const bool multi = p.in_ch > 1 || p.out_ch > 1;
+        const float* __restrict__ gin = p.in + (size_t)stream * p.in_stride + t0;
+        float* __restrict__ gout = p.out + (size_t)stream * p.out_stride + t0;
+        for (int f = 0; f < tc; f++)
+        {
+          float x_scalar = sio[tid * (kLstmChunk + 1) + f];
+          const float* w = sw;
+          for (int l = 0; l < p.num_layers; l++)
+          {
+            const int I = (l == 0) ? p.input_size : H;
+            const int W = I + H;
+            float* hs = sstate + (l * 2) * H * kLstmThreads;
+            float* cs = hs + H * kLstmThreads;
+            const float* xprev = (l == 0) ? nullptr : sstate + ((l - 1) * 2) * H * kLstmThreads;
+            const float* b = w + 4 * H * W;
+            // ifgo = W [x ; h] + b   (lstm.cpp:36-40); rows ordered i, f, g, o
+            for (int r = 0; r < 4 * H; r++)
+            {
+              const float* wr = w + r * W;
+              float acc = 0.0f;
+              if (l == 0 && !multi)
+                acc = fmaf(wr[0], x_scalar, acc); // input_size == 1
+              else if (l == 0)
+                for (int j = 0; j < I; j++)
+                  acc = fmaf(wr[j], __ldg(gin + (size_t)j * p.n_frames + f), acc);
+              else
+                for (int j = 0; j < I; j++)
+                  acc = fmaf(wr[j], xprev[j * kLstmThreads + tid], acc);
+              for (int j = 0; j < H; j++)
+                acc = fmaf(wr[I + j], hs[j * kLstmThreads + tid], acc);
+              sgate[r * kLstmThreads + tid] = acc + b[r];
+            }
+            for (int i = 0; i < H; i++)
+            {
+              const float gi = sgate[(i)*kLstmThreads + tid];
+              const float gf = sgate[(H + i) * kLstmThreads + tid];
+              const float gg = sgate[(2 * H + i) * kLstmThreads + tid];
+              const float go = sgate[(3 * H + i) * kLstmThreads + tid];
+              const float c = lstm_sigmoid(gf, p.fast_tanh) * cs[i * kLstmThreads + tid]
+                              + lstm_sigmoid(gi, p.fast_tanh) * lstm_tanh(gg, p.fast_tanh); // lstm.cpp:50-53,61-63
+              cs[i * kLstmThreads + tid] = c;
+              hs[i * kLstmThreads + tid] = lstm_sigmoid(go, p.fast_tanh) * lstm_tanh(c, p.fast_tanh); // :55-57,65-66
+            }
+            w = b + 4 * H;
+          }
+          // head (lstm.cpp:164-167)
+          const float* hl = sstate + ((p.num_layers - 1) * 2) * H * kLstmThreads;
+          if (multi)
+          {
+            // head: (out_channels x H) row-major, then the bias vector (lstm.cpp:79-97)
+            for (int oc = 0; oc < p.out_ch; oc++)
+            {
+              float y = 0.0f;
+              for (int j = 0; j < H; j++)
+                y = fmaf(w[oc * H + j], hl[j * kLstmThreads + tid], y);
+              gout[(size_t)oc * p.n_frames + f] = y + w[p.out_ch * H + oc];
+            }
+            continue;
+          }
+          float y = 0.0f;
+          for (int j = 0; j < H; j++)
+            y = fmaf(w[j], hl[j * kLstmThreads + tid], y);
+          sout[tid * (kLstmChunk + 1) + f] = y + w[H];
+        }
+      }
+      __syncthreads();
+      for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
+      {
+        const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
+        if (t0 + f < frames_of(s) && p.out_ch == 1 && p.in_ch == 1)
+          p.out[(size_t)(stream0 + s) * p.out_stride + t0 + f] = sout[s * (kLstmChunk + 1) + f];
+      }
+      __syncthreads();
     }
-    __syncthreads();
-    for (int idx = tid; idx < kLstmThreads * kLstmChunk; idx += kLstmThreads)
-    {
-      const int s = idx / kLstmChunk, f = idx - s * kLstmChunk;
-      if (t0 + f < frames_of(s) && p.out_ch == 1 && p.in_ch == 1)
-        p.out[(size_t)(stream0 + s) * p.out_stride + t0 + f] = sout[s * (kLstmChunk + 1) + f];
-    }
-    __syncthreads();
   }
   if (active)
     for (int i = 0; i < n_state; i++)
@@ -527,10 +562,12 @@ struct nam_b200_model
   bool slots_used = false;
   int n_out_of_phase = 0; // streams whose history does not end at t_base (Linear: or sits in the other buffer)
   size_t refs_capacity = 0;
-  // model bank (nam_b200_create_bank_*): bank_size >= 2 WaveNets of one WaveNetPlan, each stream bound to one of them.
-  // d_weights holds their blobs weight_stride floats apart, d_head_scales their output scales, d_bank_headers their record
-  // headers.  State rows max_batch .. max_batch + bank_size - 1 are the models' fresh rows: reset prewarms them together
-  // and copies them out; reset_streams / assign_streams copy them again.  Their histories end at fresh_clock.
+  // model bank (nam_b200_create_bank_*): bank_size >= 2 WaveNets of one WaveNetPlan, or LSTMs of one shape, each stream
+  // bound to one of them.  d_weights holds their blobs weight_stride floats apart, d_head_scales the WaveNets' output
+  // scales, d_bank_headers their record headers.  State rows max_batch .. max_batch + bank_size - 1 are the models' fresh
+  // rows: reset prewarms them together (a WaveNet bank then copies them out; an LSTM's streams keep their running state);
+  // reset_streams / assign_streams copy them.  Their histories end at fresh_clock.  An LSTM bank's rows were prewarmed in
+  // the fast-tanh regime rows_fast_tanh; a switch rebuilds them before the next copy.
   // Ordinary handles: bank_size 1, stream_model all 0, no extra rows.
   int bank_size = 1;
   std::vector<ModelSpec> bank_specs; // model k's document (bank_size entries; bank_specs[0] is `spec`'s twin)
@@ -540,6 +577,7 @@ struct nam_b200_model
   float* d_head_scales = nullptr;
   uint32_t* d_bank_headers = nullptr;
   uint32_t fresh_clock = 0;
+  int rows_fast_tanh = -1;
   unsigned char* d_xfer = nullptr; // staging of host records, scratch rows of copies and LSTM prewarms
   size_t xfer_bytes = 0;
   // staging
@@ -1458,6 +1496,10 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   kp.in_ch = m->spec.in_channels;
   kp.out_ch = m->spec.out_channels;
   kp.slots = slots;
+  // a model bank: the BANK instantiations, which read each position's model from the table (whose host copy is
+  // m->h_slots[0, batch)); the kernel family is the one an ordinary handle of the same shape gets
+  const bool bank = m->bank_size > 1;
+  kp.weight_stride = m->weight_stride;
   const int H = ls.hidden;
   if (H <= kLstmGroupMaxHidden && ls.num_layers <= kLstmGroupMaxLayers && kp.in_ch == 1 && kp.out_ch == 1)
   {
@@ -1470,10 +1512,43 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
       const int W = ((l == 0) ? ls.input_size : H) + H;
       w_floats += (size_t)4 * H * (W | 1) + 4 * H;
     }
-    const size_t smem_g = (w_floats + H + 1 + (size_t)2 * spc * (kLstmGroupChunk + 1)) * sizeof(float);
+    const size_t io_floats = (size_t)2 * spc * (kLstmGroupChunk + 1);
+    const size_t smem_g = (w_floats + H + 1 + io_floats) * sizeof(float);
     if (smem_g <= 227 * 1024)
     {
       const int grid_g = (batch + spc - 1) / spc;
+      if (bank)
+      {
+        const void* kern = G == 4 ? (const void*)lstm_group_kernel<4, true>
+                         : G == 8 ? (const void*)lstm_group_kernel<8, true>
+                         : G == 16 ? (const void*)lstm_group_kernel<16, true> : (const void*)lstm_group_kernel<32, true>;
+        // model copies: the most distinct models any CTA of this launch holds, capped by what fits beside the I/O tiles
+        // and the kernel's static table of the CTA's models
+        cudaFuncAttributes fa{};
+        CUDA_CHECK(cudaFuncGetAttributes(&fa, kern));
+        const size_t budget = 227 * 1024 - fa.sharedSizeBytes, copy_floats = w_floats + H + 1;
+        const int fit = (int)std::min<size_t>((budget / sizeof(float) - io_floats) / copy_floats, (size_t)spc);
+        if (fit < 1)
+          throw std::runtime_error("LSTM bank: one model's weights do not fit in shared memory beside the bank's model table");
+        kp.bank_copies = 1;
+        for (int b0 = 0; b0 < batch && kp.bank_copies < fit; b0 += spc)
+        {
+          int seen[kLstmGroupThreads / 4], n = 0;
+          for (int b = b0; b < std::min(batch, b0 + spc); b++)
+          {
+            const int k = m->h_slots[(size_t)b].model;
+            if (std::find(seen, seen + n, k) == seen + n)
+              seen[n++] = k;
+          }
+          kp.bank_copies = std::min(std::max(kp.bank_copies, n), fit);
+        }
+        ensure_max_dynamic_smem(kern, m->device, (int)budget);
+        void* args[] = {&kp};
+        CUDA_CHECK(cudaLaunchKernel(kern, dim3(grid_g), dim3(kLstmGroupThreads), args,
+                                    (kp.bank_copies * copy_floats + io_floats) * sizeof(float), st));
+        m->launches++;
+        return;
+      }
       auto launch = [&](auto kern) {
         CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         kern<<<grid_g, kLstmGroupThreads, smem_g, st>>>(kp);
@@ -1493,11 +1568,27 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   const size_t smem = (((m->n_weight_floats + 3) & ~(size_t)3) + (size_t)ls.num_layers * 2 * H * kLstmThreads
                        + (size_t)4 * H * kLstmThreads + (size_t)2 * kLstmThreads * (kLstmChunk + 1))
                       * sizeof(float);
-  ensure_max_dynamic_smem(reinterpret_cast<const void*>(lstm_kernel), m->device, 227 * 1024);
+  const int grid = (batch + kLstmThreads - 1) / kLstmThreads;
+  if (bank)
+  {
+    // (the kernel's static table of the CTA's models comes out of the same 227 KB)
+    const void* kern = reinterpret_cast<const void*>(lstm_kernel<true>);
+    cudaFuncAttributes fa{};
+    CUDA_CHECK(cudaFuncGetAttributes(&fa, kern));
+    const size_t budget = 227 * 1024 - fa.sharedSizeBytes;
+    if (smem > budget)
+      throw std::runtime_error("LSTM bank: one model's weights and state tiles do not fit in shared memory beside the bank's "
+                               "model table");
+    ensure_max_dynamic_smem(kern, m->device, (int)budget);
+    lstm_kernel<true><<<grid, kLstmThreads, smem, st>>>(kp);
+    CUDA_CHECK(cudaGetLastError());
+    m->launches++;
+    return;
+  }
+  ensure_max_dynamic_smem(reinterpret_cast<const void*>(lstm_kernel<false>), m->device, 227 * 1024);
   if (smem > 227 * 1024)
     throw std::runtime_error("LSTM too large for the shared-memory resident kernel");
-  const int grid = (batch + kLstmThreads - 1) / kLstmThreads;
-  lstm_kernel<<<grid, kLstmThreads, smem, st>>>(kp);
+  lstm_kernel<false><<<grid, kLstmThreads, smem, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
 }
@@ -1751,6 +1842,34 @@ int state_rows(const nam_b200_model* m)
   return m->opts.max_batch + (m->bank_size > 1 ? m->bank_size : 0);
 }
 
+// model k's document (a bank's; model 0 of an ordinary handle is its own)
+const ModelSpec& model_spec(const nam_b200_model* m, int k)
+{
+  return m->bank_size > 1 ? m->bank_specs[(size_t)k] : m->spec;
+}
+
+// an LSTM's trained initial state (lstm.cpp:24-28) as one state row: per layer h0[H] | c0[H]
+void lstm_initial_row(const ModelSpec& s, float* row)
+{
+  const int H = s.lstm.hidden;
+  for (int l = 0; l < s.lstm.num_layers; l++)
+  {
+    std::copy(s.lstm.cells[l].h0.begin(), s.lstm.cells[l].h0.end(), row + (size_t)l * 2 * H);
+    std::copy(s.lstm.cells[l].c0.begin(), s.lstm.cells[l].c0.end(), row + (size_t)l * 2 * H + H);
+  }
+}
+
+// rows [r0, r0 + n) of `state` take the h0 / c0 of models[i] (a bank's model rows; the rows of a reset_streams call)
+void write_lstm_initial_rows(nam_b200_model* m, float* state, size_t r0, const std::vector<int32_t>& models)
+{
+  const size_t stride = (size_t)m->state_stride;
+  std::vector<float> h(models.size() * stride, 0.0f);
+  for (size_t i = 0; i < models.size(); i++)
+    lstm_initial_row(model_spec(m, models[i]), h.data() + i * stride);
+  // (h is pageable: the copy stages it before returning)
+  CUDA_CHECK(cudaMemcpyAsync(state + r0 * stride, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+}
+
 void init_state(nam_b200_model* m)
 {
   const size_t total = (size_t)m->state_stride * state_rows(m);
@@ -1758,16 +1877,12 @@ void init_state(nam_b200_model* m)
   CUDA_CHECK(cudaMemsetAsync(m->d_state, 0, total * sizeof(float), m->stream));
   if (m->spec.arch == Arch::LSTM)
   {
-    // h0 / c0 are trained parameters (lstm.cpp:24-28): stream 0 gets them, then broadcast
-    std::vector<float> st((size_t)m->state_stride, 0.0f);
-    const int H = m->spec.lstm.hidden;
-    for (int l = 0; l < m->spec.lstm.num_layers; l++)
-    {
-      std::copy(m->spec.lstm.cells[l].h0.begin(), m->spec.lstm.cells[l].h0.end(), st.begin() + (size_t)l * 2 * H);
-      std::copy(m->spec.lstm.cells[l].c0.begin(), m->spec.lstm.cells[l].c0.end(), st.begin() + (size_t)l * 2 * H + H);
-    }
-    CUDA_CHECK(cudaMemcpyAsync(m->d_state, st.data(), st.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    // h0 / c0 are trained parameters (lstm.cpp:24-28): every stream starts from its model's, as every reference DSP object
+    // does (prewarm_on_reset = 0 runs no prewarm to broadcast them); a bank's model row k from model k's
+    std::vector<int32_t> models(m->stream_model);
+    for (int k = 0; k < (m->bank_size > 1 ? m->bank_size : 0); k++)
+      models.push_back(k);
+    write_lstm_initial_rows(m, m->d_state, 0, models);
   }
   if (m->spec.arch == Arch::Linear && m->d_state_tmp)
     CUDA_CHECK(cudaMemsetAsync(m->d_state_tmp, 0, total * sizeof(float), m->stream));
@@ -1803,8 +1918,8 @@ void prewarm(nam_b200_model* m)
   // DSP::prewarm continues from the instance's CURRENT state (dsp.cpp:67-101).  Straight after init_state every stream
   // would compute the same thing: stream 0 runs, its state is broadcast.  Once the streams have seen different audio
   // (a standalone nam_b200_prewarm, or a Reset of an LSTM, which keeps its running state) all of them are prewarmed.
-  // (a bank's streams run different models: nam_b200_reset prewarms it through prewarm_bank, a standalone prewarm runs
-  // every stream with its own model)
+  // (a bank's streams run different models: nam_b200_reset prewarms it through prewarm_bank or prewarm_lstm_bank, a
+  // standalone prewarm runs every stream with its own model)
   const bool identical = m->streams_identical && m->bank_size == 1;
   const int nb = identical ? 1 : m->opts.max_batch;
   CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)nb * bs * ci * sizeof(float), m->stream));
@@ -1965,7 +2080,8 @@ void copy_rows(nam_b200_model* m, float* dst, const StreamRef* dst_refs, const f
 }
 
 // nam_b200_reset for an LSTM keeps h, c and prewarms on top (fresh: from h0 / c0, like a new handle): the listed streams'
-// rows are gathered into scratch, prewarmed there exactly like prewarm() (zeros in max_frames blocks), scattered back
+// rows are gathered into scratch, prewarmed there exactly like prewarm() (zeros in max_frames blocks), scattered back.  A
+// bank's launches carry a table of the rows' models.
 void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fresh)
 {
   const size_t row = (size_t)m->state_stride;
@@ -1977,16 +2093,10 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
   const StreamRef* d_refs = upload_refs(m, refs, m->stream);
   if (fresh)
   {
-    std::vector<float> h((size_t)n * row, 0.0f);
-    const int H = m->spec.lstm.hidden;
+    std::vector<int32_t> models((size_t)n);
     for (int i = 0; i < n; i++)
-      for (int l = 0; l < m->spec.lstm.num_layers; l++)
-      {
-        float* r = h.data() + (size_t)i * row + (size_t)l * 2 * H;
-        std::copy(m->spec.lstm.cells[l].h0.begin(), m->spec.lstm.cells[l].h0.end(), r);
-        std::copy(m->spec.lstm.cells[l].c0.begin(), m->spec.lstm.cells[l].c0.end(), r + H);
-      }
-    CUDA_CHECK(cudaMemcpyAsync(rows, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+      models[(size_t)i] = m->stream_model[(size_t)streams[i]];
+    write_lstm_initial_rows(m, rows, 0, models);
   }
   else
     copy_rows(m, rows, nullptr, m->d_state, d_refs, n, m->stream);
@@ -1998,7 +2108,21 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
     ensure_staging(m, (size_t)n * bs * std::max(ci, co));
     CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
     for (int done = 0; done < ps; done += bs)
-      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, rows);
+    {
+      const StreamRef* slots = nullptr;
+      if (m->bank_size > 1)
+      {
+        for (int i = 0; i < n; i++)
+          m->h_slots[(size_t)i] = StreamRef{i, 0u, m->stream_model[(size_t)streams[i]], bs};
+        slots = push_slots(m, n, m->stream);
+      }
+      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, rows, slots);
+      if (slots)
+      {
+        CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
+        m->slots_used = true;
+      }
+    }
   }
   copy_rows(m, m->d_state, d_refs, rows, nullptr, n, m->stream);
   mark_written(m, streams, n);
@@ -2007,8 +2131,11 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
 // ---- model banks: fresh state per model --------------------------------------------------------------------------------
 // The listed streams take the fresh row of the model they are bound to (one row-copy launch whatever the mix); their
 // histories then end at fresh_clock.  A bank's calls carry every stream's clock, so the streams need not be in step.
+void prewarm_lstm_bank(nam_b200_model* m, bool streams);
 void bank_fan_out(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t st)
 {
+  if (m->spec.arch == Arch::LSTM && m->rows_fast_tanh != m->fast_tanh_runtime)
+    prewarm_lstm_bank(m, false);
   std::vector<StreamRef> refs((size_t)2 * n);
   for (int i = 0; i < n; i++)
   {
@@ -2049,6 +2176,66 @@ void prewarm_bank(nam_b200_model* m)
   for (int s = 0; s < m->opts.max_batch; s++)
     all[(size_t)s] = s;
   bank_fan_out(m, all.data(), m->opts.max_batch, m->stream);
+  CUDA_CHECK(cudaStreamSynchronize(m->stream));
+}
+
+// Why the CUDA path cannot serve this LSTM ("" when it can)
+std::string lstm_refusal(const ModelSpec& s)
+{
+  const LstmSpec& ls = s.lstm;
+  if (ls.input_size != s.in_channels) // lstm.cpp:74,111: in_channels samples land in an input_size vector
+    return "LSTM input_size (" + std::to_string(ls.input_size) + ") != in_channels (" + std::to_string(s.in_channels) + ")";
+  if ((int)ls.head_b.size() != s.out_channels || s.out_channels > 64)
+    return "LSTM head with " + std::to_string(ls.head_b.size()) + " rows for " + std::to_string(s.out_channels) + " output channels";
+  if (ls.num_layers < 1)
+    return "LSTM with zero layers";
+  return "";
+}
+
+// the LSTM kernels' weights: per layer W[4H][I+H] | b[4H]; then head_w | head_b
+std::vector<float> lstm_blob(const ModelSpec& s)
+{
+  std::vector<float> blob;
+  for (const auto& c : s.lstm.cells)
+  {
+    blob.insert(blob.end(), c.w.begin(), c.w.end());
+    blob.insert(blob.end(), c.b.begin(), c.b.end());
+  }
+  blob.insert(blob.end(), s.lstm.head_w.begin(), s.lstm.head_w.end());
+  blob.insert(blob.end(), s.lstm.head_b.begin(), s.lstm.head_b.end());
+  return blob;
+}
+
+// Reset of an LSTM bank.  An LSTM keeps h, c across Reset, so each stream (streams = true) is prewarmed in place with its
+// own model, as prewarm() does on an ordinary handle; in the same launches the K model rows restart from their models'
+// h0 / c0 and are prewarmed: each becomes the state of a freshly created and reset handle of its model, at the current
+// max_frames and prewarm_on_reset.  streams = false rebuilds the model rows alone (after a fast-tanh switch).
+void prewarm_lstm_bank(nam_b200_model* m, bool streams)
+{
+  const int K = m->bank_size, B = m->opts.max_batch;
+  std::vector<int32_t> models((size_t)K);
+  for (int k = 0; k < K; k++)
+    models[(size_t)k] = k;
+  write_lstm_initial_rows(m, m->d_state, (size_t)B, models);
+  const int ps = m->spec.prewarm_samples;
+  if (m->opts.prewarm_on_reset && ps > 0)
+  {
+    const int bs = std::max(m->max_frames, 1), n0 = streams ? B : 0, n = n0 + K;
+    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
+    ensure_staging(m, (size_t)n * bs * std::max(ci, co));
+    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
+    for (int done = 0; done < ps; done += bs)
+    {
+      for (int i = 0; i < n; i++) // streams 0 .. n0 - 1, then the model rows
+        m->h_slots[(size_t)i] = i < n0 ? StreamRef{i, m->stream_clock[(size_t)i], m->stream_model[(size_t)i], bs}
+                                       : StreamRef{B + i - n0, m->fresh_clock, i - n0, bs};
+      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, nullptr, push_slots(m, n, m->stream));
+      CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
+      m->slots_used = true;
+    }
+  }
+  m->rows_fast_tanh = m->fast_tanh_runtime;
+  m->streams_identical = false;
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 
@@ -2178,23 +2365,13 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
       case Arch::LSTM:
       {
         const LstmSpec& ls = m->spec.lstm;
-        if (ls.input_size != m->spec.in_channels) // lstm.cpp:74,111: in_channels samples land in an input_size vector
-          return fail(NAM_B200_ERR_UNSUPPORTED, "LSTM input_size (" + std::to_string(ls.input_size) + ") != in_channels ("
-                                                  + std::to_string(m->spec.in_channels) + ")");
-        if ((int)ls.head_b.size() != m->spec.out_channels || m->spec.out_channels > 64)
-          return fail(NAM_B200_ERR_UNSUPPORTED, "LSTM head with " + std::to_string(ls.head_b.size()) + " rows for "
-                                                  + std::to_string(m->spec.out_channels) + " output channels");
-        if (ls.num_layers < 1)
-          return fail(NAM_B200_ERR_UNSUPPORTED, "LSTM with zero layers");
+        const std::string why = lstm_refusal(m->spec);
+        if (!why.empty())
+          return fail(NAM_B200_ERR_UNSUPPORTED, why);
         double macs = 0.0;
         for (const auto& c : ls.cells)
-        {
-          blob.insert(blob.end(), c.w.begin(), c.w.end());
-          blob.insert(blob.end(), c.b.begin(), c.b.end());
           macs += 4.0 * c.hidden * (c.input_size + c.hidden);
-        }
-        blob.insert(blob.end(), ls.head_w.begin(), ls.head_w.end());
-        blob.insert(blob.end(), ls.head_b.begin(), ls.head_b.end());
+        blob = lstm_blob(m->spec);
         macs += (double)ls.hidden * m->spec.out_channels;
         m->state_stride = ((long)ls.num_layers * 2 * ls.hidden + 3) & ~3L;
         m->flops_per_frame = 2.0 * macs;
@@ -2599,9 +2776,10 @@ int check_ragged_args(const nam_b200_model* m, const char* fn, const int32_t* st
 constexpr size_t kRecordStagingBytes = (size_t)64 << 20;
 
 // ---- model banks: which documents can share one handle ---------------------------------------------------------------
-// Every model must be served by the fused WaveNet kernel, and models 1.. must match model 0 in everything but their weights
-// (head_scale, the last weight, included): the same WaveNetPlan apart from the blob's values, the same config object, the
-// same expected sample rate (as ContainerModel requires of its sub-models).
+// Model 0 chooses the family: WaveNets served by the fused kernel, or LSTMs.  Models 1.. must be of model 0's architecture
+// and match it in everything but their weights (a WaveNet's head_scale, the last weight, and an LSTM's h0 / c0 and head
+// included): the same expected sample rate (as ContainerModel requires of its sub-models), the same config object, and for
+// a WaveNet the same WaveNetPlan apart from the blob's values, for an LSTM the same channels, layers and sizes.
 struct BankCheck
 {
   int code = NAM_B200_OK;
@@ -2671,6 +2849,33 @@ std::string bank_difference(int k, const ModelSpec& s, const WaveNetPlan& p, con
   return "";
 }
 
+// "" when LSTM k (spec s) matches model 0 (s0), else the first difference
+std::string lstm_bank_difference(int k, const ModelSpec& s, const ModelSpec& s0)
+{
+  const std::string mk = "model " + std::to_string(k) + " differs from model 0 in ";
+  auto differ = [&](const std::string& field, double a, double b) {
+    return mk + field + " (" + json::number_to_string(a) + " vs " + json::number_to_string(b) + ")";
+  };
+  if (!(s.sample_rate == s0.sample_rate))
+    return differ("expected sample_rate", s.sample_rate, s0.sample_rate);
+  const struct
+  {
+    const char* name;
+    int v, v0;
+  } fields[] = {{"prewarm samples", s.prewarm_samples, s0.prewarm_samples},
+                {"in_channels", s.in_channels, s0.in_channels},
+                {"out_channels", s.out_channels, s0.out_channels},
+                {"num_layers", s.lstm.num_layers, s0.lstm.num_layers},
+                {"input_size", s.lstm.input_size, s0.lstm.input_size},
+                {"hidden_size", s.lstm.hidden, s0.lstm.hidden}};
+  for (const auto& f : fields)
+    if (f.v != f.v0)
+      return differ(f.name, f.v, f.v0);
+  if (s.config_fingerprint != s0.config_fingerprint)
+    return mk + "its config object (apart from the weights)";
+  return "";
+}
+
 BankCheck check_bank(const std::vector<ModelSpec>& specs)
 {
   BankCheck r;
@@ -2681,6 +2886,26 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
   };
   if (specs.empty())
     return refuse(NAM_B200_ERR_INVALID_ARGUMENT, "n_models must be >= 1");
+  if (specs[0].arch == Arch::LSTM)
+  {
+    for (size_t k = 0; k < specs.size(); k++)
+    {
+      const std::string mk = "model " + std::to_string(k) + ": ";
+      if (specs[k].arch != Arch::LSTM)
+        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + specs[k].architecture
+                                                  + ": a bank's models share model 0's architecture (LSTM)");
+      const std::string why = lstm_refusal(specs[k]); // (what an ordinary handle of the model would refuse)
+      if (!why.empty())
+        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + why);
+    }
+    for (size_t k = 1; k < specs.size(); k++)
+    {
+      const std::string d = lstm_bank_difference((int)k, specs[k], specs[0]);
+      if (!d.empty())
+        return refuse(NAM_B200_ERR_MODEL, d);
+    }
+    return r;
+  }
   for (size_t k = 0; k < specs.size(); k++)
   {
     const ModelSpec& s = specs[k];
@@ -2688,9 +2913,12 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     if (s.arch == Arch::Container)
       return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture: a slimmable document (SlimmableContainer or slimmable "
                                                    "WaveNet); a bank serves plain WaveNets of the fused kernel family");
+    if (s.arch == Arch::LSTM)
+      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture LSTM: a bank's models share model 0's architecture ("
+                                                + specs[0].architecture + ")");
     if (s.arch != Arch::WaveNet)
-      return refuse(NAM_B200_ERR_UNSUPPORTED,
-                    mk + "architecture " + s.architecture + ": a bank serves WaveNets of the fused kernel family only");
+      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + s.architecture
+                                                + ": a bank serves WaveNets of the fused kernel family or LSTMs only");
     WaveNetPlan plan = plan_wavenet(s);
     if (plan.eligible && !(s.in_channels == 1 && s.out_channels == 1))
     {
@@ -2716,31 +2944,39 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
   return r;
 }
 
-// A bank handle: an ordinary handle of model 0 on the precompiled kernels, then the blobs, output scales, record headers
-// and model rows of all K models
+// A bank handle: an ordinary handle of model 0 on the precompiled kernels, then the blobs, output scales (WaveNet), record
+// headers and model rows of all K models
 void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const std::vector<WaveNetPlan>& plans)
 {
   const int K = (int)specs.size();
+  const bool lstm = m->spec.arch == Arch::LSTM;
   m->bank_size = K;
-  m->weight_stride = (long)((m->plan.blob.size() + 3) & ~(size_t)3); // (float4 loads of every blob)
+  // (float4 loads of every blob)
+  m->weight_stride = (long)(((lstm ? m->n_weight_floats : m->plan.blob.size()) + 3) & ~(size_t)3);
   std::vector<float> blobs((size_t)K * m->weight_stride, 0.0f), scales((size_t)K);
   for (int k = 0; k < K; k++)
   {
-    std::copy(plans[(size_t)k].blob.begin(), plans[(size_t)k].blob.end(), blobs.begin() + (size_t)k * m->weight_stride);
-    scales[(size_t)k] = plans[(size_t)k].head_scale;
+    const std::vector<float> blob = lstm ? lstm_blob(specs[(size_t)k]) : plans[(size_t)k].blob;
+    std::copy(blob.begin(), blob.end(), blobs.begin() + (size_t)k * m->weight_stride);
+    if (!lstm)
+      scales[(size_t)k] = plans[(size_t)k].head_scale;
   }
   CUDA_CHECK(cudaFree(m->d_weights));
   m->d_weights = nullptr;
   CUDA_CHECK(cudaMalloc(&m->d_weights, blobs.size() * sizeof(float)));
   CUDA_CHECK(cudaMemcpy(m->d_weights, blobs.data(), blobs.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)K * sizeof(float)));
-  CUDA_CHECK(cudaMemcpy(m->d_head_scales, scales.data(), (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
+  if (!lstm)
+  {
+    CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)K * sizeof(float)));
+    CUDA_CHECK(cudaMemcpy(m->d_head_scales, scales.data(), (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
+  }
   // the model rows behind the streams' rows
   CUDA_CHECK(cudaFree(m->d_state));
   m->d_state = nullptr;
   CUDA_CHECK(cudaMalloc(&m->d_state, (size_t)m->state_stride * state_rows(m) * sizeof(float)));
-  // slot tables of up to max(max_batch, K) positions (prewarm_bank runs the K model rows in one launch)
-  const size_t n_slots = (size_t)std::max(m->opts.max_batch, K);
+  // slot tables of up to max(max_batch, K) positions (prewarm_bank runs the K model rows in one launch); an LSTM bank's
+  // Reset runs the streams and the model rows in one launch
+  const size_t n_slots = lstm ? (size_t)m->opts.max_batch + K : (size_t)std::max(m->opts.max_batch, K);
   m->h_slots.assign(n_slots, StreamRef{0, 0u, 0, 0});
   CUDA_CHECK(cudaFree(m->d_slots));
   m->d_slots = nullptr;
@@ -3200,7 +3436,9 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
       init_state(m);
     m->is_reset = true;
     CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-    if (m->opts.prewarm_on_reset)
+    if (m->bank_size > 1 && m->spec.arch == Arch::LSTM)
+      prewarm_lstm_bank(m, true); // (also rebuilds the model rows when prewarm_on_reset = 0: h0 / c0)
+    else if (m->opts.prewarm_on_reset)
       (m->bank_size > 1 ? prewarm_bank : prewarm)(m);
     CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
     // every stream is now in the state of a freshly reset one: keep stream 0's record for nam_b200_reset_streams (an LSTM
@@ -3247,7 +3485,7 @@ int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int
       rc = check_stream_list(m, streams, n, "streams", true);
     if (rc != NAM_B200_OK || n == 0)
       return rc;
-    if (m->spec.arch == Arch::LSTM)
+    if (m->spec.arch == Arch::LSTM && !(m->bank_size > 1 && fresh))
       lstm_reset_rows(m, streams, n, fresh != 0);
     else if (m->bank_size > 1)
       bank_fan_out(m, streams, n, m->stream); // each stream's own model's fresh row

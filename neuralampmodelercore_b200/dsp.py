@@ -469,7 +469,8 @@ class DSP:
 
     def assign_streams(self, streams, models) -> None:
         """Bind streams[i] to model models[i] and give it that model's freshly reset state; other streams are untouched.
-        On an ordinary handle, models all 0 is reset_streams."""
+        On an ordinary handle, models all 0 is reset_streams (for an LSTM: fresh=False, which keeps the running state); on
+        a bank of K >= 2 it is reset_streams(fresh=True) on an ordinary handle of the new model."""
         s = self._streams(streams)
         k = np.ascontiguousarray(np.broadcast_to(np.asarray(models, dtype=np.int32), s.shape), dtype=np.int32)
         self._check(self._lib.nam_b200_assign_streams(self._h, self._i32p(s), len(s), self._i32p(k)))
@@ -552,8 +553,11 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
                  fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
                  tile_mode: int = 0, jit: int = 0) -> DSP:
     """A model bank: one handle of `batch` streams over the K documents in `configs` (paths, dicts or JSON texts), which
-    must share one shape (bank_check).  Every stream starts bound to model 0; DSP.assign_streams rebinds.  The options are
-    get_dsp's; jit = 1 is refused for K >= 2, and a bank of one document is get_dsp."""
+    must share one shape (bank_check): WaveNets of the fused kernel family, or LSTMs.  Every stream starts bound to model
+    0; DSP.assign_streams rebinds.  Each stream behaves as the same stream of an ordinary jit=2 handle of its model: an LSTM
+    bank's Reset keeps each stream's running state and prewarms it with its own model, reset_streams(fresh=False) does
+    the same for the listed streams, and fresh=True gives them their model's h0 / c0 plus the prewarm.  The options are
+    get_dsp's; jit = 1 and kernel_geometry = 4 are refused for K >= 2, and a bank of one document is get_dsp."""
     lib = _capi.load()
     o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit)
     arr, _keep = _text_array(_documents(configs))
@@ -565,8 +569,10 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
 
 
 def bank_check(configs) -> dict:
-    """Host-only: can these documents share a bank?  {ok, n_models, reason (first offending model and field),
-    fingerprints (each model's state record fingerprint)}.  Needs no GPU."""
+    """Host-only: can these documents share a bank?  Model 0 chooses the family (fused-kernel WaveNets or LSTMs); the
+    others must match it in everything but their weights -- for LSTMs: sample rate, in/out channels, num_layers,
+    input_size, hidden_size and the config object.  {ok, n_models, reason (first offending model and field), fingerprints
+    (each model's state record fingerprint)}.  Needs no GPU."""
     import json
 
     lib = _capi.load()

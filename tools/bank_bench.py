@@ -9,12 +9,19 @@ slot mixes models, the worst case for blob reloads).  Arms:
   jit2      one ordinary handle of model 0 with jit = 2: the precompiled-kernel ceiling;
   jit       one ordinary handle of model 0 with the default jit: the model-specialised kernel a bank gives up.
 
+--arch lstm runs the same workloads on LSTM banks instead (rows carry "shape"): "lstm" = lstm.nam reweighted per model
+(the lane-group kernel, G = 4: 32 streams per CTA) and "h70" = a random one-layer cell of hidden size 70 (one thread per
+stream, 64 streams per CTA, one pass per distinct model of a CTA).  The thread-per-stream kernel takes ~1 s per
+4096-frame call of 4096 such streams, so h70 runs only calls of up to --h70-max-frames frames; the others print "not
+measured".  LSTM handles are made with prewarm off (Reset's 24000-sample prewarm is not what is timed).
+
 Before timing, every K checks the bank's first call against fresh ordinary handles of its models at the timed sizes (up to
 --check-models models; the bank's row reports bytes_equal and max_abs_diff, and the run stops above 1e-5).  Each arm is timed over --iters calls after --warmup, the arms alternated --repeats
 times; the rate is Msamples/s (streams x frames / s) with the spread (min..max) of the repeats.  Prints the card's name and
 power limit first, then one JSON line per (K, frames, binding, arm).
 
-    python tools/bank_bench.py [--ks 1 8 64 512] [--frames 64 4096] [--iters 10] [--warmup 2] [--repeats 3]
+    python tools/bank_bench.py [--arch wavenet|lstm] [--ks 1 8 64 512] [--frames 64 4096] [--iters 10] [--warmup 2]
+                               [--repeats 3]
 """
 from __future__ import annotations
 
@@ -40,12 +47,17 @@ def card() -> str:
         return "unknown (nvidia-smi unavailable)"
 
 
-def family(k: int) -> list:
+def family(k: int, shape: str = "a1") -> list:
     import numpy as np
 
     from tests import nam_fixtures as fx
 
-    base = fx.load_model("wavenet_a1_standard")
+    if shape == "h70":
+        return [{"version": "0.5.4", "architecture": "LSTM", "sample_rate": 48000.0,
+                 "config": {"input_size": 1, "hidden_size": 70, "num_layers": 1},
+                 "weights": [float(v) for v in np.random.default_rng(i).uniform(-0.3, 0.3, 4 * 70 * 71 + 4 * 70 + 2 * 70 + 71)]}
+                for i in range(k)]
+    base = fx.load_model({"a1": "wavenet_a1_standard", "lstm": "lstm"}[shape])
     w0 = np.asarray(base["weights"], np.float32)
     docs = []
     for i in range(k):
@@ -66,6 +78,8 @@ def main() -> None:
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--handles-max-k", type=int, default=64)
     ap.add_argument("--check-models", type=int, default=8)
+    ap.add_argument("--arch", choices=["wavenet", "lstm"], default="wavenet")
+    ap.add_argument("--h70-max-frames", type=int, default=64)
     args = ap.parse_args()
     os.environ.setdefault("NAM_B200_JIT_CACHE", tempfile.mkdtemp(prefix="nam_b200_jit_"))  # (the tree may be read-only)
 
@@ -100,29 +114,47 @@ def main() -> None:
         r0, r1 = rows
         return lambda: d.process_batch_device(x[r0].data_ptr(), y[r0].data_ptr(), r1 - r0, n_frames, F, F, cuda_stream=cs)
 
+    for shape in (["a1"] if args.arch == "wavenet" else ["lstm", "h70"]):
+        run_shape(args, shape, B, F, x, y, stream, timed, device_call)
+
+
+def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
+    import numpy as np
+
+    import neuralampmodelercore_b200 as nb
+
+    tag = {} if shape == "a1" else {"shape": shape}  # (the WaveNet rows keep their fields)
+    opts = {} if shape == "a1" else {"prewarm": False}
     singles = {}
     for jit in (2, 0):
-        d = nb.get_dsp(family(1)[0], batch=B, jit=jit)
+        d = nb.get_dsp(family(1, shape)[0], batch=B, jit=jit, **opts)
         d.Reset(48000.0, F)
         singles[jit] = d
 
     for K in args.ks:
-        docs = family(K)
-        bank = nb.get_dsp_bank(docs, batch=B, jit=2)
+        docs = family(K, shape)
+        bank = nb.get_dsp_bank(docs, batch=B, jit=2, **opts)
         bank.Reset(48000.0, F)
         per = B // K
         handles = []
         if K <= args.handles_max_k and K > 1:
             for d in docs:
-                h = nb.get_dsp(d, batch=per, jit=2)
+                h = nb.get_dsp(d, batch=per, jit=2, **opts)
                 h.Reset(48000.0, F)
                 handles.append(h)
         for binding in ("grouped", "round_robin"):
             models = np.arange(B) // per if binding == "grouped" else np.arange(B) % K
             models = np.minimum(models, K - 1).astype(np.int32)
             for n_frames in args.frames:
+                if shape == "h70" and n_frames > args.h70_max_frames:
+                    for a in ("bank", "handles", "jit2", "jit"):
+                        print(json.dumps({**tag, "K": K, "frames": n_frames, "binding": binding, "arm": a,
+                                          "msamples_per_s": None, "note": "not measured"}), flush=True)
+                    continue
                 bank.Reset(48000.0, F)
                 bank.assign_streams(np.arange(B), models)
+                if shape != "a1":  # (an LSTM keeps h, c across Reset: every stream restarts from its model's h0 / c0)
+                    bank.reset_streams(np.arange(B), fresh=True)
                 # correctness at the timed size: the bank's first call against fresh ordinary handles of its models
                 bank_run = device_call(bank, (0, B), n_frames)
                 bank_run()
@@ -132,7 +164,7 @@ def main() -> None:
                 check = {"max_abs_diff": 0.0, "bytes_equal": True}
                 for k in range(min(K, args.check_models)):
                     rows = np.nonzero(models == k)[0]
-                    h = nb.get_dsp(docs[k], batch=len(rows), jit=2)
+                    h = nb.get_dsp(docs[k], batch=len(rows), jit=2, **opts)
                     h.Reset(48000.0, F)
                     want = h.process_batch(np.ascontiguousarray(xs[rows]))
                     h.close()
@@ -154,7 +186,7 @@ def main() -> None:
                         ms = timed(run, args.iters)
                         rates[a].append(B * n_frames / (ms * 1e-3) / 1e6)
                 for a in ("bank", "handles", "jit2", "jit"):
-                    row = {"K": K, "frames": n_frames, "binding": binding, "arm": a}
+                    row = {**tag, "K": K, "frames": n_frames, "binding": binding, "arm": a}
                     if a in rates:
                         r = sorted(rates[a])
                         row.update(msamples_per_s=round(r[len(r) // 2], 1), spread=[round(r[0], 1), round(r[-1], 1)])
