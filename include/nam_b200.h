@@ -169,20 +169,38 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
 /* ---- model banks: one handle, streams of different captures of one architecture ----------------------------------------
  * A bank is a handle created from K >= 1 .nam documents of one shape; each of its max_batch streams is bound to one of the
  * K models, and every process call runs each listed stream with its own model's weights, in the launches an ordinary
- * handle's call of that batch takes.  Which documents can share a bank -- model 0 chooses one of two families:
- *   - WaveNets served by the fused kernel family (wavenet.nam, a1_standard, A2-Lite and A2-Full shapes): not the general
- *     kernel (gated, FiLM, ...), SlimmableContainer files or slimmable WaveNets.  Models 1.. equal model 0 in everything
+ * handle's call of that batch takes.  Which documents can share a bank -- model 0 chooses one of four families:
+ *   - WaveNets served by the fused kernel family (wavenet.nam, a1_standard, A2-Lite and A2-Full shapes); not
+ *     SlimmableContainer files or slimmable WaveNets.  Models 1.. equal model 0 in everything
  *     but their weights: layer arrays, channels, kernel sizes, dilations, activations and their parameters, hence the
  *     packed kernel layout and blob length; the config object apart from its unused head_scale field (head_scale is the
  *     last weight, so it is per model); the expected sample rate.
+ *   - WaveNets an ordinary handle serves with the general kernel (gating, FiLM, grouped convolutions, head1x1, bottleneck !=
+ *     channels, a condition_dsp sub-model, a post-stack head, multi-channel in / out).  Models 1.. equal model 0 in the
+ *     expected sample rate and prewarm length, every array and layer field (channels, bottleneck, kernel sizes, dilations,
+ *     groups, gating mode, activations, FiLM sites, layer1x1 / head1x1), the post-stack head, the condition_dsp's shape,
+ *     hence the general kernel's descriptors and blob length, and the config object.  Both output scales (the network's
+ *     and the condition_dsp's head_scale) are weights, so they are per model; a nested condition_dsp document's weights,
+ *     metadata and version are per model too.
+ *   - ConvNets an ordinary handle serves.  Models 1.. equal model 0 in the sample rate, channels, dilations, BatchNorm
+ *     presence, activation, in / out channels and the config object; the folded BatchNorm is per model.
  *   - LSTMs an ordinary handle serves (a model it would refuse is refused with its reason).  Models 1.. equal model 0 in
  *     the expected sample rate (hence the prewarm length), in_channels and out_channels, num_layers, input_size,
  *     hidden_size and the config object; their weights, trained h0 / c0 and head are per model.
- *   ConvNet, Linear and mixed families are refused.  Refusals (NAM_B200_ERR_UNSUPPORTED for a model outside the family,
- *   NAM_B200_ERR_MODEL for a mismatch) name the first offending model index and the field.  jit = 1 is refused (a
- *   model-specialised kernel compiles one model's weights into its code); jit = 0 or 3 silently keeps the precompiled
- *   kernels, and nam_b200_jit_note says so.  kernel_geometry 4 (the general kernel) is refused.  A bank of one document is
- *   exactly nam_b200_create_from_json / _from_file, JIT included.
+ *   Linear and mixed families are refused: a WaveNet on the fused kernel with one on the general kernel (either order) is
+ *   refused with "model k: kernel: ...", naming model 0's family.  Refusals (NAM_B200_ERR_UNSUPPORTED for a model outside
+ *   the family, NAM_B200_ERR_MODEL for a mismatch) name the first offending model index and the field.  jit:
+ *   - fused and LSTM banks: jit = 1 is refused (a model-specialised kernel compiles one model's weights into its code);
+ *     jit = 0 or 3 silently keeps the precompiled kernels, and nam_b200_jit_note says so;
+ *   - general-WaveNet banks: jit as on an ordinary handle, for the general kernel compiled for the bank's SHAPE (the
+ *     descriptors are compiled in, each stream's weights are staged in shared memory; nam_b200_bank_jit_prepare_json):
+ *     0 = default (on at max_batch >= 256), 1 = required (creation fails with the reason when it cannot be had, e.g. a
+ *     blob over 200 KB), 2 = off, 3 = preferred.  jit_state and nam_b200_jit_note report it;
+ *   - ConvNet banks: as an ordinary ConvNet handle (there is no compiled ConvNet kernel).
+ *   kernel_geometry 4 (the general kernel) is refused for fused-family and LSTM banks; on a general-WaveNet bank it selects
+ *   the precompiled general kernel (as on an ordinary handle), any other non-zero geometry is taken as 4, and a ConvNet bank
+ *   ignores it as an ordinary ConvNet handle does.  A bank of one document is exactly nam_b200_create_from_json /
+ *   _from_file, JIT included.
  * All streams start bound to model 0.  Every call of this header works on a bank, each stream exactly (bit for bit) as the
  * same stream of an ordinary jit = 2 handle of its model:
  *   - process calls (nam_b200_process_f32 and _device, process_streams*, the ragged calls, the planar DSP::process on stream
@@ -200,14 +218,16 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
  *     and an ordinary handle of its model in either direction;
  *   - nam_b200_set_fast_tanh: as on an ordinary handle (an LSTM bank rebuilds its model rows in the new regime before the
  *     next fresh-state copy).
- * Device memory: the K blobs (a1_standard: ~14k floats each; lstm.nam: 64 floats each) and, for WaveNets,
- * K output scales, plus K "model rows" of state_stride floats each (a1_standard: 196 KB each; lstm.nam: 8 floats) that
+ * Device memory: the K blobs (a1_standard: ~14k floats each; lstm.nam: 64 floats each; a general WaveNet's blob carries
+ * its two output scales behind its weights, wavenet_a2_max: ~1.9k floats) and, for fused-family WaveNets, K output scales,
+ * plus K "model rows" of state_stride floats each (a1_standard: 196 KB each; lstm.nam: 8 floats) that
  * hold every model's freshly reset state (an LSTM's: h0 / c0 plus the prewarm): reset prewarms them together -- an LSTM
  * bank in the same launches as its streams -- and reset_streams and assign_streams copy them (one launch whatever the mix).
  * Cost of mixing: an LSTM kernel's CTA holds several streams (lane groups: 128 / G of them; thread per stream: 64); the
  * lane-group kernel keeps one weight copy per distinct model of a CTA where they fit and makes another pass where they do
  * not, the thread-per-stream kernel makes one pass per distinct model (up to 64 with round-robin binding).  Keep a model's
- * streams in adjacent slots. */
+ * streams in adjacent slots.  The general WaveNet and ConvNet kernels run one stream per CTA at a time: a CTA restages the
+ * blob into shared memory only when its next stream's model differs. */
 int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const nam_b200_options* opts, nam_b200_model** out);
 int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out);
 /* K of a bank; 1 for every other handle (so model index 0 is valid on every handle). */
@@ -229,6 +249,12 @@ int nam_b200_bank_model_info(const nam_b200_model* m, int k, nam_b200_info* info
  * 64-bit integer as in nam_b200_state_layout_json).  Returns 0 whatever
  * the verdict; NAM_B200_ERR_INVALID_ARGUMENT when the buffer is too small. */
 int nam_b200_bank_check_json(const char* const* texts, int n_models, char* out, int64_t capacity);
+/* Host-only, no CUDA: compile (or find in the cache) the general kernel compiled for the shape of a bank of general-kernel
+ * WaveNets (the kernel such a bank runs under jit 0 / 1 / 3), as nam_b200_jit_prepare_json does for one model.  The cache
+ * key holds no weight, so every bank of one shape shares the cubin.  A JSON object: ok, from_cache, compile_seconds,
+ * cubin_bytes, threads, smem_bytes (one blob), why_not.  Refused like nam_b200_create_bank_from_json, and for every other
+ * family with NAM_B200_ERR_UNSUPPORTED. */
+int nam_b200_bank_jit_prepare_json(const char* const* texts, int n_models, int fast_tanh, char* out, int64_t capacity);
 
 /* Batched throughput entry: `batch` (<= max_batch) streams, stream b reads
  * in[b*in_stride .. +n_frames) and writes out[b*out_stride .. +n_frames); n_frames <= max_frames.

@@ -8,6 +8,7 @@ from ._build import build, LIB_PATH  # noqa: F401
 from .dsp import (  # noqa: F401
     DSP,
     bank_check,
+    bank_jit_prepare,
     CudaUnavailableError,
     NamFileValidationError,
     UnsupportedModelError,
@@ -31,6 +32,7 @@ __all__ = [
     "get_dsp",
     "get_dsp_bank",
     "bank_check",
+    "bank_jit_prepare",
     "inspect",
     "jit_prepare",
     "submodels",

@@ -112,6 +112,7 @@ EXPORTED_SYMBOLS = [
     "nam_b200_stream_models",
     "nam_b200_bank_model_info",
     "nam_b200_bank_check_json",
+    "nam_b200_bank_jit_prepare_json",
 ]
 
 
@@ -208,6 +209,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_stream_models.argtypes = [vp, i32p, C.c_int, i32p]
     lib.nam_b200_bank_model_info.argtypes = [vp, C.c_int, C.POINTER(Info)]
     lib.nam_b200_bank_check_json.argtypes = [strv, C.c_int, C.c_char_p, C.c_int64]
+    lib.nam_b200_bank_jit_prepare_json.argtypes = [strv, C.c_int, C.c_int, C.c_char_p, C.c_int64]
+    lib.nam_b200_bank_jit_prepare_json.restype = C.c_int
     for name in ("nam_b200_create_bank_from_json", "nam_b200_create_bank_from_files", "nam_b200_bank_size",
                  "nam_b200_assign_streams", "nam_b200_stream_models", "nam_b200_bank_model_info", "nam_b200_bank_check_json"):
         getattr(lib, name).restype = C.c_int

@@ -100,6 +100,7 @@ struct ConvNetKernelParams
   uint32_t t_base;
   int n_weight_floats;
   const StreamRef* slots; // nullptr: position i is state row i at t_base; else row slots[i].stream at slots[i].clock
+  long weight_stride; // model bank (the BANK instantiation): position i runs the blob at weights + slots[i].model * weight_stride
 };
 
 struct GenericKernelParams
@@ -118,6 +119,10 @@ struct GenericKernelParams
   uint32_t t_base;
   int n_weight_floats; // multiple of 4; the kernel keeps the blob in shared memory when it was given the room
   const StreamRef* slots; // as ConvNetKernelParams::slots
+  // model bank (the BANK instantiation): position i runs the blob at weights + slots[i].model * weight_stride, whose floats
+  // scale_off and scale_off + 1 are that model's net.head_scale and cond.head_scale (the GNets' head_scale is not read)
+  long weight_stride;
+  int scale_off;
 };
 
 } // namespace namb200

@@ -43,6 +43,10 @@ struct JitParams
   // slot table (nullptr: position b is state row b at t_base, running n_frames frames): position b uses row slots[b].stream
   // at slots[b].clock and runs slots[b].frames frames; inputs and outputs stay indexed by position
   const StreamRef* slots;
+  // model bank (wavenet_generic_spec_kernel compiled for a bank's shape, gspec::bank): position b runs the blob at
+  // weights + slots[b].model * weight_stride; every other kernel ignores these
+  const float* weights;
+  long weight_stride;
 };
 
 // wavenet_lat_kernel's parameter: the same, plus the completion doorbell (done_flag may be null): a word in mapped host

@@ -558,20 +558,38 @@ bool finite_desc(const GenericPlan& gp)
 }
 } // namespace
 
-std::string generic_spec_header_source(const GenericPlan& gp)
+std::string generic_spec_header_source(const GenericPlan& gp, const bool bank)
 {
   std::ostringstream o;
-  o << "// generated by jit_spec.cpp: one WaveNet with the reference's full option set, as compile-time data\n"
+  o << "// generated by jit_spec.cpp: one WaveNet" << (bank ? " shape (a model bank's)" : "")
+    << " with the reference's full option set, as compile-time data\n"
        "#define NAMB200_GSPEC_HEADER_INCLUDED 1\n#include \"generic_desc.h\"\nnamespace gspec {\nusing namespace namb200;\n";
   o << "constexpr int has_cond = " << (gp.has_cond ? 1 : 0) << ";\n";
-  o << "__device__ constexpr GNet net = " << lit(gp.net) << ";\n";
-  o << "__device__ constexpr GNet cond = " << lit(gp.has_cond ? gp.cond : GNet{}) << ";\n";
+  // (a bank's header carries no weight: its output scales are cleared here and read from each model's blob)
+  GNet net = gp.net, cond = gp.has_cond ? gp.cond : GNet{};
+  if (bank)
+    net.head_scale = cond.head_scale = 0.0f;
+  o << "__device__ constexpr GNet net = " << lit(net) << ";\n";
+  o << "__device__ constexpr GNet cond = " << lit(cond) << ";\n";
   o << "__device__ constexpr GLayer layers[" << std::max<size_t>(gp.layers.size(), 1) << "] = {\n";
   for (const GLayer& L : gp.layers)
     o << "  " << lit(L) << ",\n";
   if (gp.layers.empty())
     o << "  {}\n";
-  o << "};\n__device__ const unsigned Wb[" << std::max<size_t>(gp.weights.size(), 1) << "] = {\n";
+  if (bank)
+  {
+    // w(i): the current stream's blob, staged in dynamic shared memory by the kernel; the two output scales follow the
+    // weights in the blob (nam_b200.cu setup_bank)
+    o << "};\nconstexpr int bank = 1;\nconstexpr int blob_floats = " << generic_bank_blob_floats(gp) << ";\n"
+      << "constexpr int scale_off = " << gp.weights.size() << ";\n"
+      << "extern __shared__ float4 blob4[];\n"
+      << "__device__ __forceinline__ float w(const int i) { return reinterpret_cast<const float*>(blob4)[i]; }\n"
+      << "__device__ __forceinline__ float out_scale(const int c) { return w(scale_off + c); }\n}  // namespace gspec\n";
+    return o.str();
+  }
+  o << "};\nconstexpr int bank = 0;\nconstexpr int blob_floats = 0;\nextern __shared__ float4 blob4[];  // (no blob to stage)\n"
+    << "__device__ __forceinline__ float out_scale(const int c) { return c ? cond.head_scale : net.head_scale; }\n";
+  o << "__device__ const unsigned Wb[" << std::max<size_t>(gp.weights.size(), 1) << "] = {\n";
   char buf[16];
   for (size_t i = 0; i < gp.weights.size(); i++)
   {
@@ -586,7 +604,12 @@ std::string generic_spec_header_source(const GenericPlan& gp)
   return o.str();
 }
 
-SpecBuild build_generic_spec_kernel(const GenericPlan& gp)
+size_t generic_bank_blob_floats(const GenericPlan& gp)
+{
+  return (gp.weights.size() + 2 + 3) & ~(size_t)3;
+}
+
+SpecBuild build_generic_spec_kernel(const GenericPlan& gp, const bool bank)
 {
   SpecBuild r;
   r.geom.nt = kGenTile;
@@ -605,7 +628,13 @@ SpecBuild build_generic_spec_kernel(const GenericPlan& gp)
     r.why_not = "too many weights to unroll (" + std::to_string(gp.weights.size()) + ")";
     return r;
   }
-  const CompiledKernel ck = compile_or_fetch("wavenet_generic_spec", generic_spec_header_source(gp), "wavenet_generic_spec.cuh",
+  if (bank && generic_bank_blob_floats(gp) * sizeof(float) > kGenericBankSmemBytes)
+  {
+    r.why_not = "one model's weights (" + std::to_string(generic_bank_blob_floats(gp) * sizeof(float))
+                + " bytes) exceed the shared memory of the shape-compiled kernel";
+    return r;
+  }
+  const CompiledKernel ck = compile_or_fetch("wavenet_generic_spec", generic_spec_header_source(gp, bank), "wavenet_generic_spec.cuh",
                                              kGenericSpecKernelSource, "NAM_B200_GSPEC_SOURCE", {},
                                              {{"generic_desc.h", kGenericDescSource}});
   r.ok = ck.ok;

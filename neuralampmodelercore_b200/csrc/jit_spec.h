@@ -57,8 +57,15 @@ SpecBuild build_lat_kernel(const WaveNetPlan& plan, int frame_warps);
 
 /// The general kernel (every WaveNet option of the reference) compiled for one model: wavenet_generic_spec.cuh with the
 /// descriptors of generic_desc.h and the weights as constant data.  Entry point: wavenet_generic_spec_kernel, 128 threads.
-std::string generic_spec_header_source(const GenericPlan& gp);
-SpecBuild build_generic_spec_kernel(const GenericPlan& gp);
+/// bank = true: the kernel compiled for the SHAPE of a model bank's general WaveNets -- the descriptors as constants, no
+/// weights: gspec::w(i) reads the current stream's blob (generic_bank_blob_floats floats: the weights, then the net's and
+/// the condition_dsp's output scales) from dynamic shared memory, which the kernel stages when the stream's model changes.
+/// The header holds no weight, so every bank of one shape shares one cubin.  Unavailable when a blob exceeds
+/// kGenericBankSmemBytes.
+std::string generic_spec_header_source(const GenericPlan& gp, bool bank = false);
+SpecBuild build_generic_spec_kernel(const GenericPlan& gp, bool bank = false);
+size_t generic_bank_blob_floats(const GenericPlan& gp);
+constexpr size_t kGenericBankSmemBytes = 200 * 1024;
 
 /// The same for a small mono LSTM (lstm_spec.cuh: one thread per stream, weights as FFMA immediates); the cubin holds
 /// lstm_spec_kernel_exact and lstm_spec_kernel_fast (the fast-tanh switch is read at run time, lstm.cpp:48).

@@ -1172,7 +1172,8 @@ void setup_lat_kernel(nam_b200_model* m)
 JitParams jit_params(const nam_b200_model* m, float* state, const float* d_in, float* d_out, long in_stride, long out_stride,
                      int batch, int n_frames, const StreamRef* slots)
 {
-  return JitParams{state, m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, m->t_base, slots};
+  return JitParams{state,      m->state_stride, d_in, d_out, in_stride, out_stride, batch, n_frames, m->t_base, slots,
+                   m->d_weights, m->weight_stride};
 }
 
 void launch_wavenet_lat(nam_b200_model* m, const JitParams& jp, cudaStream_t st)
@@ -1205,8 +1206,10 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   if (m->use_generic && m->gen_spec_kernel != nullptr && m->opts.kernel_geometry == 0)
   {
     void* args[] = {&jp};
+    // (a bank's shape-compiled kernel stages each stream's blob in dynamic shared memory)
+    const size_t smem = m->bank_size > 1 ? (size_t)m->weight_stride * sizeof(float) : 0;
     CUDA_CHECK(cudaLaunchKernel((const void*)m->gen_spec_kernel, dim3(std::max(1, std::min(batch, 16 * m->sm_count))), dim3(kGenTile),
-                                args, 0, st));
+                                args, smem, st));
     m->launches++;
     return;
   }
@@ -1228,17 +1231,23 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
     gp.batch = batch;
     gp.n_frames = n_frames;
     gp.t_base = m->t_base;
-    gp.n_weight_floats = (int)((m->n_weight_floats + 3) & ~(size_t)3);
+    // (a bank: each model's blob with its two output scales behind the weights; its calls always carry a table)
+    const bool bank = m->bank_size > 1;
+    gp.n_weight_floats = bank ? (int)m->weight_stride : (int)((m->n_weight_floats + 3) & ~(size_t)3);
+    gp.weight_stride = m->weight_stride;
+    gp.scale_off = (int)m->gplan.weights.size();
     const size_t wbytes = (size_t)gp.n_weight_floats * sizeof(float);
     const int grid_g = std::min(batch, 16 * m->sm_count);
     if (wbytes <= 200 * 1024)
     {
-      auto kern = slots ? wavenet_generic_kernel<true, true> : wavenet_generic_kernel<true>;
+      auto kern = bank ? wavenet_generic_kernel<true, true, true>
+                       : (slots ? wavenet_generic_kernel<true, true> : wavenet_generic_kernel<true>);
       ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
       kern<<<grid_g, kGenTile, wbytes, st>>>(gp);
     }
     else
-      (slots ? wavenet_generic_kernel<false, true> : wavenet_generic_kernel<false>)<<<grid_g, kGenTile, 0, st>>>(gp);
+      (bank ? wavenet_generic_kernel<false, true, true>
+            : (slots ? wavenet_generic_kernel<false, true> : wavenet_generic_kernel<false>))<<<grid_g, kGenTile, 0, st>>>(gp);
     CUDA_CHECK(cudaGetLastError());
     m->launches++;
     return;
@@ -1449,6 +1458,32 @@ void setup_generic_spec_kernel(nam_b200_model* m)
     return jit_unavailable(m, why, b.ok);
   m->spec_state = 1;
   m->spec_note = "general kernel, " + jit_loaded_note(b);
+}
+
+// A general-family bank: the general kernel compiled for the bank's shape (no weights in its code; each stream's blob is staged
+// in shared memory), under the handle's jit policy.  Called once the bank's blobs are in place (setup_bank).
+void setup_generic_bank_kernel(nam_b200_model* m)
+{
+  if (!jit_wanted(m) || m->opts.kernel_geometry == 4)
+    return;
+  const SpecBuild b = build_generic_spec_kernel(m->gplan, true);
+  std::string why = b.why_not;
+  if (b.ok)
+  {
+    std::string err = m->spec_lib.load(b.cubin);
+    if (err.empty())
+      err = m->spec_lib.kernel(&m->gen_spec_kernel, "wavenet_generic_spec_kernel", (size_t)m->weight_stride * sizeof(float),
+                               kGenTile, &m->spec_ctas_per_sm);
+    if (err.empty() && m->spec_ctas_per_sm < 1)
+      err = "the shape-compiled general kernel does not fit on an SM";
+    if (!err.empty())
+      why = "loading the shape-compiled general kernel failed: " + err;
+  }
+  if (!why.empty())
+    return jit_unavailable(m, "model bank of " + std::to_string(m->bank_size) + " models: " + why, b.ok);
+  m->spec_state = 1;
+  m->spec_note = "model bank of " + std::to_string(m->bank_size) + " models: the general kernel compiled for the bank's shape, "
+                 + jit_loaded_note(b);
 }
 
 // `state`: rows of per-stream state to run on (nullptr = the handle's d_state; nam_b200_reset_streams prewarms a gathered
@@ -1674,16 +1709,19 @@ void launch_convnet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   kp.t_base = m->t_base;
   kp.n_weight_floats = (int)((m->n_weight_floats + 3) & ~(size_t)3);
   kp.slots = slots;
+  kp.weight_stride = m->weight_stride; // (a bank: its calls always carry a table)
+  const bool bank = m->bank_size > 1;
   const size_t wbytes = (size_t)kp.n_weight_floats * sizeof(float);
   const int grid = std::min(batch, 16 * m->sm_count);
   if (wbytes <= 200 * 1024)
   {
-    auto kern = slots ? convnet_kernel<true, true> : convnet_kernel<true>;
+    auto kern = bank ? convnet_kernel<true, true, true> : (slots ? convnet_kernel<true, true> : convnet_kernel<true>);
     ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
     kern<<<grid, kGenTile, wbytes, st>>>(kp);
   }
   else
-    (slots ? convnet_kernel<false, true> : convnet_kernel<false>)<<<grid, kGenTile, 0, st>>>(kp);
+    (bank ? convnet_kernel<false, true, true>
+          : (slots ? convnet_kernel<false, true> : convnet_kernel<false>))<<<grid, kGenTile, 0, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
 }
@@ -2159,13 +2197,18 @@ void prewarm_bank(nam_b200_model* m)
   const int bs = std::max(m->max_frames, 1);
   if (ps > 0)
   {
-    ensure_staging(m, (size_t)std::max(m->opts.max_batch, K) * bs);
-    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)K * bs * sizeof(float), m->stream));
+    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
+    ensure_staging(m, (size_t)std::max(m->opts.max_batch, K) * bs * std::max(ci, co));
+    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)K * bs * ci * sizeof(float), m->stream));
     for (int done = 0; done < ps; done += bs)
     {
       for (int k = 0; k < K; k++)
         m->h_slots[(size_t)k] = StreamRef{m->opts.max_batch + k, m->t_base, k, bs};
-      launch_wavenet(m, m->d_in, m->d_out, K, bs, bs, bs, m->stream, 0, push_slots(m, K, m->stream));
+      const StreamRef* slots = push_slots(m, K, m->stream);
+      if (m->spec.arch == Arch::ConvNet)
+        launch_convnet(m, m->d_in, m->d_out, K, bs, (long)(bs * ci), (long)(bs * co), m->stream, slots);
+      else
+        launch_wavenet(m, m->d_in, m->d_out, K, bs, (long)(bs * ci), (long)(bs * co), m->stream, 0, slots);
       CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
       m->slots_used = true;
       m->t_base += (uint32_t)bs;
@@ -2776,15 +2819,26 @@ int check_ragged_args(const nam_b200_model* m, const char* fn, const int32_t* st
 constexpr size_t kRecordStagingBytes = (size_t)64 << 20;
 
 // ---- model banks: which documents can share one handle ---------------------------------------------------------------
-// Model 0 chooses the family: WaveNets served by the fused kernel, or LSTMs.  Models 1.. must be of model 0's architecture
-// and match it in everything but their weights (a WaveNet's head_scale, the last weight, and an LSTM's h0 / c0 and head
-// included): the same expected sample rate (as ContainerModel requires of its sub-models), the same config object, and for
-// a WaveNet the same WaveNetPlan apart from the blob's values, for an LSTM the same channels, layers and sizes.
+// Model 0 chooses the family: WaveNets served by the fused kernel, WaveNets served by the general kernel, ConvNets, or
+// LSTMs.  Models 1.. must be of model 0's architecture and family and match it in everything but their weights (a
+// WaveNet's head_scale, the last weight, and an LSTM's h0 / c0 and head included): the same expected sample rate (as
+// ContainerModel requires of its sub-models), the same config object, and the same packed form apart from the blob's values
+// (WaveNetPlan, GenericPlan) or, for an LSTM, the same channels, layers and sizes.
+enum class BankFamily
+{
+  Fused,
+  General,
+  ConvNet,
+  Lstm
+};
+
 struct BankCheck
 {
   int code = NAM_B200_OK;
   std::string reason; // names the first offending model and the field
-  std::vector<WaveNetPlan> plans;
+  BankFamily family = BankFamily::Fused;
+  std::vector<WaveNetPlan> plans; // fused family
+  std::vector<GenericPlan> gplans; // general WaveNets and ConvNets
 };
 
 // "" when model k (spec s, plan p) matches model 0 (s0, p0), else the first difference
@@ -2876,6 +2930,169 @@ std::string lstm_bank_difference(int k, const ModelSpec& s, const ModelSpec& s0)
   return "";
 }
 
+// "" when the WaveNet w (model k's, or its condition_dsp's) has the shape of w0, else the first difference -- the fields the
+// general kernel's descriptors are made of, named as the config names them; `at` prefixes the field ("condition_dsp ")
+std::string general_wavenet_difference(const std::string& mk, const std::string& at, const WaveNetSpec& w, const WaveNetSpec& w0)
+{
+  auto differ = [&](const std::string& field, double a, double b) {
+    return mk + at + field + " (" + json::number_to_string(a) + " vs " + json::number_to_string(b) + ")";
+  };
+  if (w.in_channels != w0.in_channels)
+    return differ("in_channels", w.in_channels, w0.in_channels);
+  if (w.arrays.size() != w0.arrays.size())
+    return differ("the number of layer arrays", (double)w.arrays.size(), (double)w0.arrays.size());
+  auto act_difference = [&](const std::string& where, const ActSpec& a, const ActSpec& a0) -> std::string {
+    if (a.type != a0.type)
+      return differ(where, (int)a.type, (int)a0.type);
+    if (a.slopes.size() != a0.slopes.size())
+      return differ(where + " PReLU slope count", (double)a.slopes.size(), (double)a0.slopes.size());
+    if (a.slope != a0.slope || a.min_val != a0.min_val || a.max_val != a0.max_val || a.min_slope != a0.min_slope
+        || a.max_slope != a0.max_slope)
+      return mk + at + where + " parameters";
+    return "";
+  };
+  for (size_t a = 0; a < w.arrays.size(); a++)
+  {
+    const ArraySpec &A = w.arrays[a], &A0 = w0.arrays[a];
+    const std::string ar = "array " + std::to_string(a) + " ";
+    const struct
+    {
+      const char* name;
+      int v, v0;
+    } fields[] = {{"input_size", A.input_size, A0.input_size},
+                  {"condition_size", A.condition_size, A0.condition_size},
+                  {"channels", A.channels, A0.channels},
+                  {"bottleneck", A.bottleneck, A0.bottleneck},
+                  {"head_size", A.head_size, A0.head_size},
+                  {"head kernel_size", A.head_kernel, A0.head_kernel},
+                  {"head dilation", A.head_dilation, A0.head_dilation},
+                  {"head_bias", A.head_bias ? 1 : 0, A0.head_bias ? 1 : 0},
+                  {"groups_input", A.groups_input, A0.groups_input},
+                  {"groups_input_mixin", A.groups_input_mixin, A0.groups_input_mixin},
+                  {"layer1x1 active", A.l1x1_active ? 1 : 0, A0.l1x1_active ? 1 : 0},
+                  {"layer1x1 groups", A.l1x1_groups, A0.l1x1_groups},
+                  {"head1x1 active", A.h1x1_active ? 1 : 0, A0.h1x1_active ? 1 : 0},
+                  {"head1x1 out_channels", A.h1x1_out, A0.h1x1_out},
+                  {"head1x1 groups", A.h1x1_groups, A0.h1x1_groups},
+                  {"number of layers (dilations)", (int)A.layers.size(), (int)A0.layers.size()}};
+    for (const auto& f : fields)
+      if (f.v != f.v0)
+        return differ(ar + f.name, f.v, f.v0);
+    for (size_t l = 0; l < A.layers.size(); l++)
+    {
+      const LayerSpec &L = A.layers[l], &L0 = A0.layers[l];
+      const std::string lt = ar + "layer " + std::to_string(l) + " ";
+      if (L.conv.kernel != L0.conv.kernel)
+        return differ(lt + "kernel_size", L.conv.kernel, L0.conv.kernel);
+      if (L.conv.dilation != L0.conv.dilation)
+        return differ(lt + "dilation", L.conv.dilation, L0.conv.dilation);
+      if (L.conv.groups != L0.conv.groups)
+        return differ(lt + "groups", L.conv.groups, L0.conv.groups);
+      if (L.gating != L0.gating)
+        return differ(lt + "gating mode", (int)L.gating, (int)L0.gating);
+      std::string d = act_difference(lt + "activation", L.act, L0.act);
+      if (d.empty() && L.gating != Gating::None)
+        d = act_difference(lt + "secondary activation", L.sec_act, L0.sec_act);
+      if (!d.empty())
+        return d;
+      for (int f = 0; f < F_COUNT; f++)
+      {
+        const FilmSpec &F = L.film[f], &F0 = L0.film[f];
+        const std::string ft = lt + "FiLM site " + std::to_string(f) + " ";
+        if (F.active != F0.active)
+          return differ(ft + "active", F.active ? 1 : 0, F0.active ? 1 : 0);
+        if (F.shift != F0.shift)
+          return differ(ft + "shift", F.shift ? 1 : 0, F0.shift ? 1 : 0);
+        if (F.groups != F0.groups)
+          return differ(ft + "groups", F.groups, F0.groups);
+      }
+    }
+  }
+  if (w.with_head != w0.with_head)
+    return differ("post-stack head", w.with_head ? 1 : 0, w0.with_head ? 1 : 0);
+  if (w.with_head)
+  {
+    const PostHeadSpec &H = w.post_head, &H0 = w0.post_head;
+    if (H.convs.size() != H0.convs.size() || H.channels != H0.channels || H.out_channels != H0.out_channels)
+      return mk + at + "the post-stack head's convolutions";
+    for (size_t i = 0; i < H.convs.size(); i++)
+      if (H.convs[i].kernel != H0.convs[i].kernel || H.convs[i].dilation != H0.convs[i].dilation)
+        return mk + at + "the post-stack head's convolutions";
+    const std::string d = act_difference("post-stack head activation", H.act, H0.act);
+    if (!d.empty())
+      return d;
+  }
+  if ((w.condition_dsp != nullptr) != (w0.condition_dsp != nullptr))
+    return differ("condition_dsp", w.condition_dsp ? 1 : 0, w0.condition_dsp ? 1 : 0);
+  if (w.condition_dsp)
+  {
+    const ModelSpec &c = *w.condition_dsp, &c0 = *w0.condition_dsp;
+    if (c.out_channels != c0.out_channels)
+      return differ("condition_dsp out_channels", c.out_channels, c0.out_channels);
+    return general_wavenet_difference(mk, at + "condition_dsp ", c.wavenet, c0.wavenet);
+  }
+  return "";
+}
+
+// "" when general WaveNet or ConvNet k (spec s, plan p) matches model 0 (s0, p0), else the first difference
+std::string general_bank_difference(int k, const ModelSpec& s, const GenericPlan& p, const ModelSpec& s0, const GenericPlan& p0)
+{
+  const std::string mk = "model " + std::to_string(k) + " differs from model 0 in ";
+  auto differ = [&](const std::string& field, double a, double b) {
+    return mk + field + " (" + json::number_to_string(a) + " vs " + json::number_to_string(b) + ")";
+  };
+  if (!(s.sample_rate == s0.sample_rate))
+    return differ("expected sample_rate", s.sample_rate, s0.sample_rate);
+  const struct
+  {
+    const char* name;
+    int v, v0;
+  } fields[] = {{"in_channels", s.in_channels, s0.in_channels}, {"out_channels", s.out_channels, s0.out_channels}};
+  for (const auto& f : fields)
+    if (f.v != f.v0)
+      return differ(f.name, f.v, f.v0);
+  bool same = p.weights.size() == p0.weights.size() && p.state_floats == p0.state_floats;
+  if (s.arch == Arch::ConvNet)
+  {
+    const ConvNetSpec &c = s.convnet, &c0 = s0.convnet;
+    if (c.channels != c0.channels)
+      return differ("channels", c.channels, c0.channels);
+    if (c.blocks.size() != c0.blocks.size())
+      return differ("the number of blocks (dilations)", (double)c.blocks.size(), (double)c0.blocks.size());
+    for (size_t b = 0; b < c.blocks.size(); b++)
+      if (c.blocks[b].conv.dilation != c0.blocks[b].conv.dilation)
+        return differ("block " + std::to_string(b) + " dilation", c.blocks[b].conv.dilation, c0.blocks[b].conv.dilation);
+    if (c.batchnorm != c0.batchnorm)
+      return differ("batchnorm", c.batchnorm ? 1 : 0, c0.batchnorm ? 1 : 0);
+    if (c.groups != c0.groups)
+      return differ("groups", c.groups, c0.groups);
+    if (c.act.type != c0.act.type)
+      return differ("activation", (int)c.act.type, (int)c0.act.type);
+    // (GConvNet is plain 4-byte fields: no padding to compare)
+    same = same && std::memcmp(&p.convnet, &p0.convnet, sizeof(GConvNet)) == 0;
+  }
+  else
+  {
+    const std::string d = general_wavenet_difference(mk, "", s.wavenet, s0.wavenet);
+    if (!d.empty())
+      return d;
+    // the packed form apart from the weights and the two output scales (which a bank's kernel reads from each blob)
+    GNet n = p.net, n0 = p0.net, c = p.cond, c0 = p0.cond;
+    n.head_scale = n0.head_scale = c.head_scale = c0.head_scale = 0.0f;
+    same = same && p.has_cond == p0.has_cond && std::memcmp(&n, &n0, sizeof(GNet)) == 0
+           && std::memcmp(&c, &c0, sizeof(GNet)) == 0 && p.layers.size() == p0.layers.size()
+           && std::memcmp(p.layers.data(), p0.layers.data(), p.layers.size() * sizeof(GLayer)) == 0;
+  }
+  // (after the fields above: the receptive field decides it)
+  if (s.prewarm_samples != s0.prewarm_samples)
+    return differ("prewarm samples", s.prewarm_samples, s0.prewarm_samples);
+  if (!same)
+    return mk + "the packed kernel layout (descriptors, rings or blob length)";
+  if (s.config_fingerprint != s0.config_fingerprint)
+    return mk + "its config object (apart from the weights and head_scale)";
+  return "";
+}
+
 BankCheck check_bank(const std::vector<ModelSpec>& specs)
 {
   BankCheck r;
@@ -2888,6 +3105,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     return refuse(NAM_B200_ERR_INVALID_ARGUMENT, "n_models must be >= 1");
   if (specs[0].arch == Arch::LSTM)
   {
+    r.family = BankFamily::Lstm;
     for (size_t k = 0; k < specs.size(); k++)
     {
       const std::string mk = "model " + std::to_string(k) + ": ";
@@ -2906,19 +3124,32 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     }
     return r;
   }
+  auto family_name = [](BankFamily f) { return f == BankFamily::Fused ? "fused" : "general"; };
   for (size_t k = 0; k < specs.size(); k++)
   {
     const ModelSpec& s = specs[k];
     const std::string mk = "model " + std::to_string(k) + ": ";
     if (s.arch == Arch::Container)
       return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture: a slimmable document (SlimmableContainer or slimmable "
-                                                   "WaveNet); a bank serves plain WaveNets of the fused kernel family");
-    if (s.arch == Arch::LSTM)
-      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture LSTM: a bank's models share model 0's architecture ("
-                                                + specs[0].architecture + ")");
-    if (s.arch != Arch::WaveNet)
+                                                   "WaveNet); a bank serves plain WaveNets, ConvNets and LSTMs");
+    if (s.arch != Arch::WaveNet && s.arch != Arch::ConvNet && s.arch != Arch::LSTM)
       return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + s.architecture
-                                                + ": a bank serves WaveNets of the fused kernel family or LSTMs only");
+                                                + ": a bank serves WaveNets, ConvNets or LSTMs only");
+    if (s.arch != specs[0].arch)
+      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + s.architecture
+                                                + ": a bank's models share model 0's architecture (" + specs[0].architecture + ")");
+    if (s.arch == Arch::ConvNet)
+    {
+      // (what an ordinary handle of the model would refuse)
+      GenericPlan gp = plan_convnet(s);
+      if (!gp.eligible)
+        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "ConvNet not supported on the CUDA path: " + gp.why_not);
+      r.family = BankFamily::ConvNet;
+      r.gplans.push_back(std::move(gp));
+      continue;
+    }
+    // the kernel an ordinary handle of the model gets by default (create_common): the fused one when the model is eligible,
+    // mono and fits its shared memory, else the general one
     WaveNetPlan plan = plan_wavenet(s);
     if (plan.eligible && !(s.in_channels == 1 && s.out_channels == 1))
     {
@@ -2930,14 +3161,33 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
       plan.eligible = false;
       plan.why_not = "packed weights + tile exceed the shared memory of the fused kernel";
     }
+    BankFamily f = BankFamily::Fused;
+    GenericPlan gp;
     if (!plan.eligible)
-      return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "kernel: not served by the fused WaveNet kernel (" + plan.why_not
-                                                + "); a bank serves the fused family only (the general kernel does not take banks)");
-    r.plans.push_back(std::move(plan));
+    {
+      gp = plan_generic(s);
+      if (!gp.eligible)
+        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "kernel: WaveNet not supported on the CUDA path: fused kernel: "
+                                                  + plan.why_not + "; general kernel: " + gp.why_not);
+      f = BankFamily::General;
+    }
+    if (k == 0)
+      r.family = f;
+    else if (f != r.family)
+      return refuse(NAM_B200_ERR_UNSUPPORTED,
+                    mk + "kernel: served by the " + family_name(f) + " kernel"
+                      + (f == BankFamily::General ? " (fused kernel: " + plan.why_not + ")" : std::string())
+                      + "; model 0 (" + family_name(r.family) + " family) chooses the bank's kernel family");
+    if (f == BankFamily::Fused)
+      r.plans.push_back(std::move(plan));
+    else
+      r.gplans.push_back(std::move(gp));
   }
   for (size_t k = 1; k < specs.size(); k++)
   {
-    const std::string d = bank_difference((int)k, specs[k], r.plans[k], specs[0], r.plans[0]);
+    const std::string d = r.family == BankFamily::Fused
+                            ? bank_difference((int)k, specs[k], r.plans[k], specs[0], r.plans[0])
+                            : general_bank_difference((int)k, specs[k], r.gplans[k], specs[0], r.gplans[0]);
     if (!d.empty())
       return refuse(NAM_B200_ERR_MODEL, d);
   }
@@ -2946,26 +3196,40 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
 
 // A bank handle: an ordinary handle of model 0 on the precompiled kernels, then the blobs, output scales (WaveNet), record
 // headers and model rows of all K models
-void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const std::vector<WaveNetPlan>& plans)
+void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const BankCheck& bc)
 {
   const int K = (int)specs.size();
-  const bool lstm = m->spec.arch == Arch::LSTM;
+  const bool lstm = bc.family == BankFamily::Lstm, fused = bc.family == BankFamily::Fused;
   m->bank_size = K;
-  // (float4 loads of every blob)
-  m->weight_stride = (long)(((lstm ? m->n_weight_floats : m->plan.blob.size()) + 3) & ~(size_t)3);
+  // model k's blob: the fused family's packed blob (its output scale goes to d_head_scales), an LSTM's weights, or the
+  // general kernel's weights -- a general WaveNet's followed by its net and condition_dsp output scales, which the BANK
+  // instantiation reads from the blob (float4 loads of every blob)
+  auto blob_of = [&](int k) {
+    if (lstm)
+      return lstm_blob(specs[(size_t)k]);
+    if (fused)
+      return bc.plans[(size_t)k].blob;
+    const GenericPlan& gp = bc.gplans[(size_t)k];
+    std::vector<float> b = gp.weights;
+    if (m->spec.arch == Arch::WaveNet)
+      b.insert(b.end(), {gp.net.head_scale, gp.cond.head_scale});
+    return b;
+  };
+  const size_t len0 = blob_of(0).size();
+  m->weight_stride = (long)((len0 + 3) & ~(size_t)3);
   std::vector<float> blobs((size_t)K * m->weight_stride, 0.0f), scales((size_t)K);
   for (int k = 0; k < K; k++)
   {
-    const std::vector<float> blob = lstm ? lstm_blob(specs[(size_t)k]) : plans[(size_t)k].blob;
+    const std::vector<float> blob = blob_of(k);
     std::copy(blob.begin(), blob.end(), blobs.begin() + (size_t)k * m->weight_stride);
-    if (!lstm)
-      scales[(size_t)k] = plans[(size_t)k].head_scale;
+    if (fused)
+      scales[(size_t)k] = bc.plans[(size_t)k].head_scale;
   }
   CUDA_CHECK(cudaFree(m->d_weights));
   m->d_weights = nullptr;
   CUDA_CHECK(cudaMalloc(&m->d_weights, blobs.size() * sizeof(float)));
   CUDA_CHECK(cudaMemcpy(m->d_weights, blobs.data(), blobs.size() * sizeof(float), cudaMemcpyHostToDevice));
-  if (!lstm)
+  if (fused)
   {
     CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)K * sizeof(float)));
     CUDA_CHECK(cudaMemcpy(m->d_head_scales, scales.data(), (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
@@ -2992,6 +3256,8 @@ void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const std::ve
   m->spec_state = 0;
   m->spec_note = "model bank of " + std::to_string(K) + " models: the precompiled kernels, which read each stream's weights as "
                  "data (a model-specialised kernel compiles one model's weights into its code)";
+  if (bc.family == BankFamily::General)
+    setup_generic_bank_kernel(m); // (throws under jit = 1 when the shape-compiled kernel cannot be had)
   init_state(m);
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
@@ -3008,19 +3274,29 @@ int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opt
     std::memcpy(&o, user_opts, std::min<size_t>(sizeof o, (size_t)std::max(user_opts->struct_size, 0)));
     o.struct_size = sizeof o;
   }
-  if (o.jit == 1)
+  if (o.jit == 1 && (bc.family == BankFamily::Fused || bc.family == BankFamily::Lstm))
     return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: jit = 1 (required) cannot be met: a model-specialised kernel compiles "
                                           "one model's weights into its code, a bank's streams each bring their own");
-  if (o.kernel_geometry == 4)
-    return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: kernel_geometry 4 (the general kernel) does not take banks");
-  o.jit = 2; // jit 0 / 3: the precompiled kernels, silently (nam_b200_jit_note says why)
+  if (o.kernel_geometry == 4 && (bc.family == BankFamily::Fused || bc.family == BankFamily::Lstm))
+    return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: kernel_geometry 4 (the general kernel) does not take banks of the fused "
+                                          "WaveNet or LSTM families (model 0 chooses the family)");
+  // Fused and LSTM banks: jit 0 / 3 run the precompiled kernels, silently (nam_b200_jit_note says why).  General banks: model
+  // 0's handle is made without its model-specialised kernel, then setup_bank applies the requested jit to the kernel compiled
+  // for the bank's shape.  ConvNet banks take jit as an ordinary ConvNet handle does (it has no compiled kernel).
+  const int user_jit = o.jit;
+  if (bc.family != BankFamily::ConvNet)
+    o.jit = 2;
+  if (bc.family == BankFamily::General && o.kernel_geometry != 0)
+    o.kernel_geometry = 4; // (the general kernel is the family's: a fused geometry must not move model 0 onto the fused kernel)
   nam_b200_model* h = nullptr;
   const int rc = create_common(ModelSpec(specs[0]), &o, &h);
   if (rc != NAM_B200_OK)
     return rc;
   std::unique_ptr<nam_b200_model> m(h);
+  if (bc.family == BankFamily::General)
+    m->opts.jit = user_jit;
   const int rc2 = guarded(m.get(), [&]() -> int {
-    setup_bank(m.get(), std::move(specs), bc.plans);
+    setup_bank(m.get(), std::move(specs), bc);
     return NAM_B200_OK;
   });
   if (rc2 == NAM_B200_OK)
@@ -3788,6 +4064,48 @@ int nam_b200_bank_check_json(const char* const* texts, int n_models, char* out, 
   if ((int64_t)s.size() >= capacity)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "the bank check needs " + std::to_string(s.size() + 1) + " bytes, the buffer has "
                                                  + std::to_string(capacity));
+  std::memcpy(out, s.c_str(), s.size() + 1);
+  return NAM_B200_OK;
+}
+
+int nam_b200_bank_jit_prepare_json(const char* const* texts, int n_models, int fast_tanh, char* out, int64_t capacity)
+{
+  if (!out || capacity <= 0 || !texts || n_models < 1)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument, empty output buffer or n_models < 1");
+  LoadOptions lo;
+  lo.fast_tanh = fast_tanh != 0;
+  std::vector<ModelSpec> specs;
+  try
+  {
+    for (int k = 0; k < n_models; k++)
+    {
+      if (!texts[k])
+        throw std::runtime_error("model " + std::to_string(k) + ": null document");
+      specs.push_back(model_spec_from_text(texts[k], lo));
+    }
+  }
+  catch (const std::exception& ex)
+  {
+    return fail(NAM_B200_ERR_MODEL, ex.what());
+  }
+  const BankCheck bc = check_bank(specs);
+  if (bc.code != NAM_B200_OK)
+    return fail(bc.code, "model bank: " + bc.reason);
+  if (bc.family != BankFamily::General)
+    return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: only banks of general-kernel WaveNets have a shape-compiled kernel");
+  const SpecBuild b = build_generic_spec_kernel(bc.gplans[0], true);
+  std::string why;
+  for (char c : b.why_not.substr(0, 600))
+    why += (c == '"' || c == '\\') ? '\'' : (c == '\n' ? ' ' : c);
+  char buf[1024];
+  std::snprintf(buf, sizeof buf,
+                "{\"ok\": %s, \"from_cache\": %s, \"compile_seconds\": %.3f, \"cubin_bytes\": %zu, \"threads\": %d, "
+                "\"smem_bytes\": %zu, \"why_not\": \"%s\"}",
+                b.ok ? "true" : "false", b.from_cache ? "true" : "false", b.compile_seconds, b.cubin.size(), kGenTile,
+                generic_bank_blob_floats(bc.gplans[0]) * sizeof(float), why.c_str());
+  const std::string s(buf);
+  if ((int64_t)s.size() >= capacity)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "the report needs " + std::to_string(s.size() + 1) + " bytes");
   std::memcpy(out, s.c_str(), s.size() + 1);
   return NAM_B200_OK;
 }

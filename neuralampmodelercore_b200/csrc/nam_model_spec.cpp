@@ -1030,7 +1030,9 @@ uint64_t model_fingerprint(const std::string& architecture, const json::Value& c
 }
 
 // the same over the architecture and the "config" object alone, without its "head_scale" field (the reference reads the
-// scale from the last weight, model.cpp:670): equal for documents that differ in their weights only
+// scale from the last weight, model.cpp:670): equal for documents that differ in their weights only.  A nested
+// "condition_dsp" document contributes its architecture, its sample rate and its own config fingerprint: its weights,
+// metadata and version are the sub-model's data, like the outer document's.
 uint64_t config_fingerprint(const std::string& architecture, const json::Value& config)
 {
   Fnv64 f;
@@ -1049,7 +1051,16 @@ uint64_t config_fingerprint(const std::string& architecture, const json::Value& 
   for (auto* kv : members)
   {
     f.str(kv->first);
-    f.value(kv->second);
+    const json::Value& v = kv->second;
+    if (kv->first == "condition_dsp" && v.is_object() && v.contains("architecture") && v.contains("config"))
+    {
+      const json::Value& arch = v.at("architecture");
+      f.value(arch);
+      f.value(v.get("sample_rate"));
+      f.u64(config_fingerprint(arch.is_string() ? arch.as_string() : std::string(), v.at("config")));
+    }
+    else
+      f.value(v);
   }
   return f.h;
 }

@@ -258,8 +258,9 @@ __device__ __forceinline__ void g_layer(const GenThread& c, const GLayer& L, flo
 }
 
 // one frame through a whole network: in (in_channels), cond (its condition vector) -> out (out_channels)
+// (head_scale: N.head_scale, or in a bank the stream's model's, from its blob)
 __device__ __forceinline__ void g_net(const GenThread& c, const GNet& N, const GLayer* __restrict__ layers,
-                                      const float* in, const float* cond, float* out)
+                                      const float* in, const float* cond, float* out, const float head_scale)
 {
   float x[kGenMaxVec], xin[kGenMaxVec], head[kGenMaxVec], hout[kGenMaxVec];
   for (int i = 0; i < N.in_channels; i++)
@@ -283,7 +284,7 @@ __device__ __forceinline__ void g_net(const GenThread& c, const GNet& N, const G
     // post-stack head (model.cpp:854-883, Head::process :87-103): repeated activation -> Conv1D
     float cur[kGenMaxVec], nxt[kGenMaxVec];
     for (int i = 0; i < last.head_size; i++)
-      cur[i] = N.head_scale * hout[i];
+      cur[i] = head_scale * hout[i];
     for (int h = 0; h < N.n_head_convs; h++)
     {
       const GConv& V = N.head_convs[h];
@@ -298,7 +299,35 @@ __device__ __forceinline__ void g_net(const GenThread& c, const GNet& N, const G
   }
   else
     for (int i = 0; i < N.out_channels; i++)
-      out[i] = N.head_scale * hout[i];
+      out[i] = head_scale * hout[i];
+}
+
+// Model banks (BANK; a bank's calls always carry a table): position s runs the blob of model slots[s].model, at
+// weights + model * weight_stride.  With WS the CTA keeps the blob of the model it staged last and restages only when the
+// next position's model differs (the condition is uniform over the CTA, so the barriers around the copy are too).
+template <bool WS, bool BANK, typename P>
+__device__ __forceinline__ void g_bank_select(GenThread& c, const P& p, const int s, int& staged)
+{
+  if constexpr (BANK)
+  {
+    const int model = p.slots[s].model;
+    const float* __restrict__ blob = p.weights + (size_t)model * p.weight_stride;
+    if constexpr (WS)
+    {
+      if (model != staged)
+      {
+        __syncthreads(); // every thread is done with the previous model's weights
+        extern __shared__ float4 gen_smem4[];
+        const float4* src = reinterpret_cast<const float4*>(blob);
+        for (int i = threadIdx.x; i < p.n_weight_floats / 4; i += kGenTile)
+          gen_smem4[i] = __ldg(src + i);
+        __syncthreads();
+        staged = model;
+      }
+    }
+    else
+      c.w = blob;
+  }
 }
 
 // The C ABI's batched entry; persistent CTAs, one stream at a time.  Multi-channel models (model.cpp:809-820,
@@ -307,13 +336,17 @@ __device__ __forceinline__ void g_net(const GenThread& c, const GNet& N, const G
 // TBL: the call carries a slot table (its own instantiation: a call without one runs the table-free code).
 // WS: the weight blob is staged in shared memory once per CTA (it fits for every model the kernel accepts in
 // practice: example_models/wavenet_a2_max.nam is 7.5 KB); otherwise it is read through the read-only path.
-template <bool WS, bool TBL = false>
+template <bool WS, bool TBL = false, bool BANK = false>
 __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_constant__ GenericKernelParams p)
 {
+  static_assert(TBL || !BANK, "a bank's calls carry a slot table");
   extern __shared__ float4 gen_smem4[];
   GenThread c;
   c.w = p.weights;
-  if constexpr (WS)
+  int staged = -1; // BANK && WS: the model whose blob is in shared memory
+  if constexpr (BANK && WS)
+    c.w = reinterpret_cast<const float*>(gen_smem4);
+  if constexpr (WS && !BANK)
   {
     const float4* src = reinterpret_cast<const float4*>(p.weights);
     for (int i = threadIdx.x; i < p.n_weight_floats / 4; i += kGenTile)
@@ -331,6 +364,10 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
     c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
+    g_bank_select<WS, BANK>(c, p, s, staged);
+    float bank_scale[2] = {0.0f, 0.0f}; // BANK: the position's model's output scales (net, cond), read once per position
+    if constexpr (BANK)
+      bank_scale[0] = c.w[p.scale_off], bank_scale[1] = c.w[p.scale_off + 1];
     for (int t0 = 0; t0 < n; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;
@@ -340,11 +377,11 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
       for (int ch = 0; ch < ci; ch++)
         in[ch] = c.valid ? __ldg(xin + (size_t)ch * p.n_frames + f) : 0.0f;
       if (p.has_cond)
-        g_net(c, p.cond, p.layers, in, in, cond); // _process_condition (model.cpp:777-807)
+        g_net(c, p.cond, p.layers, in, in, cond, BANK ? bank_scale[1] : p.cond.head_scale); // _process_condition (model.cpp:777-807)
       else
         for (int ch = 0; ch < ci; ch++)
           cond[ch] = in[ch];
-      g_net(c, p.net, p.layers, in, cond, out);
+      g_net(c, p.net, p.layers, in, cond, out, BANK ? bank_scale[0] : p.net.head_scale);
       if (c.valid)
         for (int ch = 0; ch < co; ch++)
           yout[(size_t)ch * p.n_frames + f] = out[ch];
@@ -354,13 +391,18 @@ __global__ void __launch_bounds__(kGenTile) wavenet_generic_kernel(const __grid_
 
 // ConvNet (NAM/convnet.cpp:204-272): the same frame-per-thread tiling; a block is Conv1D(kernel 2, dilation d) ->
 // BatchNorm as two separate roundings, multiply then add (convnet.cpp:39-46) -> activation (:66-88); head W x + b.
-template <bool WS, bool TBL = false>
+// BANK: as wavenet_generic_kernel's (a ConvNet has no output scale).
+template <bool WS, bool TBL = false, bool BANK = false>
 __global__ void __launch_bounds__(kGenTile) convnet_kernel(const __grid_constant__ ConvNetKernelParams p)
 {
+  static_assert(TBL || !BANK, "a bank's calls carry a slot table");
   extern __shared__ float4 gen_smem4[];
   GenThread c;
   c.w = p.weights;
-  if constexpr (WS)
+  int staged = -1;
+  if constexpr (BANK && WS)
+    c.w = reinterpret_cast<const float*>(gen_smem4);
+  if constexpr (WS && !BANK)
   {
     const float4* src = reinterpret_cast<const float4*>(p.weights);
     for (int i = threadIdx.x; i < p.n_weight_floats / 4; i += kGenTile)
@@ -376,6 +418,7 @@ __global__ void __launch_bounds__(kGenTile) convnet_kernel(const __grid_constant
     c.st = p.state + (size_t)(TBL ? p.slots[s].stream : s) * p.state_stride;
     const float* __restrict__ xin = p.in + (size_t)s * p.in_stride;
     float* __restrict__ yout = p.out + (size_t)s * p.out_stride;
+    g_bank_select<WS, BANK>(c, p, s, staged);
     for (int t0 = 0; t0 < n; t0 += kGenTile)
     {
       const int f = t0 + (int)threadIdx.x;

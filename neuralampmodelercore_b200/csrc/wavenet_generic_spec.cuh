@@ -9,6 +9,10 @@
 // compiler unrolls the whole network into straight-line code: the vectors become registers, the descriptor fields
 // constants, the weights FFMA immediates, the option switches (gating, FiLM sites, head1x1, activations) disappear.
 //
+// Compiled for a model bank's SHAPE (gspec::bank, jit_spec.cpp), the header holds the descriptors only: gspec::w(i) reads the
+// current stream's blob from shared memory, staged when the next stream's model differs, and the output scales come from
+// the blob through gspec::out_scale (the ordinary header's returns the constant).
+//
 // What it computes (reference, under NAM/): wavenet/model.cpp:183-393 Layer::Process, :463-549 LayerArray, :777-910
 // WaveNet::process with condition_dsp, :19-103 the post-stack head; film.h:76-190; gating_activations.h:100-113,209-227.
 #pragma once
@@ -282,7 +286,7 @@ __device__ __forceinline__ void net_forward(const Th& c, const float* in, const 
     float cur[kGenMaxVec], nxt[kGenMaxVec];
 #pragma unroll
     for (int i = 0; i < last.head_size; i++)
-      cur[i] = N.head_scale * hout[i];
+      cur[i] = gspec::out_scale(COND ? 1 : 0) * hout[i];
     static_for<0, N.n_head_convs>([&](auto h_c) {
       constexpr GConv V = N.head_convs[decltype(h_c)::value];
 #pragma unroll
@@ -301,7 +305,7 @@ __device__ __forceinline__ void net_forward(const Th& c, const float* in, const 
   {
 #pragma unroll
     for (int i = 0; i < N.out_channels; i++)
-      out[i] = N.head_scale * hout[i];
+      out[i] = gspec::out_scale(COND ? 1 : 0) * hout[i];
   }
 }
 
@@ -312,8 +316,23 @@ extern "C" __global__ void __launch_bounds__(namb200_gspec::kTile) wavenet_gener
   using namespace namb200_gspec;
   Th c;
   constexpr int ci = gspec::net.in_channels, co = gspec::net.out_channels;
+  int staged = -1; // a bank's kernel: the model whose blob is in shared memory
   for (int s = blockIdx.x; s < p.batch; s += gridDim.x)
   {
+    if constexpr (gspec::bank != 0)
+    {
+      // (a bank's calls always carry a table; the condition is uniform over the CTA, so are the barriers)
+      const int model = p.slots[s].model;
+      if (model != staged)
+      {
+        __syncthreads(); // every thread is done with the previous model's weights
+        const float4* src = reinterpret_cast<const float4*>(p.weights + (size_t)model * p.weight_stride);
+        for (int i = threadIdx.x; i < gspec::blob_floats / 4; i += kTile)
+          gspec::blob4[i] = __ldg(src + i);
+        __syncthreads();
+        staged = model;
+      }
+    }
     const unsigned clock = p.slots ? p.slots[s].clock : p.t_base;
     const int n = p.slots ? p.slots[s].frames : p.n_frames; // (p.n_frames stays the channel-plane pitch)
     c.st = p.state + (size_t)(p.slots ? p.slots[s].stream : s) * p.state_stride;

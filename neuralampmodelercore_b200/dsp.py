@@ -553,11 +553,16 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
                  fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
                  tile_mode: int = 0, jit: int = 0) -> DSP:
     """A model bank: one handle of `batch` streams over the K documents in `configs` (paths, dicts or JSON texts), which
-    must share one shape (bank_check): WaveNets of the fused kernel family, or LSTMs.  Every stream starts bound to model
+    must share one shape (bank_check): WaveNets of the fused kernel family, WaveNets of the general kernel (A2-style,
+    condition_dsp, multi-channel), ConvNets, or LSTMs.  Every stream starts bound to model
     0; DSP.assign_streams rebinds.  Each stream behaves as the same stream of an ordinary jit=2 handle of its model: an LSTM
     bank's Reset keeps each stream's running state and prewarms it with its own model, reset_streams(fresh=False) does
     the same for the listed streams, and fresh=True gives them their model's h0 / c0 plus the prewarm.  The options are
-    get_dsp's; jit = 1 and kernel_geometry = 4 are refused for K >= 2, and a bank of one document is get_dsp."""
+    get_dsp's.  jit: a general-WaveNet bank takes it as an ordinary handle does, for the general kernel compiled for the
+    bank's shape (bank_jit_prepare; 0 default, 1 required, 2 off, 3 preferred); fused and LSTM banks refuse jit = 1 and
+    run the precompiled kernels under 0 / 3; a ConvNet bank takes it as an ordinary ConvNet handle.  kernel_geometry = 4
+    is refused for fused-family and LSTM banks; on a general bank it selects the precompiled general kernel, and a
+    ConvNet bank ignores it.  A bank of one document is get_dsp."""
     lib = _capi.load()
     o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit)
     arr, _keep = _text_array(_documents(configs))
@@ -569,9 +574,12 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
 
 
 def bank_check(configs) -> dict:
-    """Host-only: can these documents share a bank?  Model 0 chooses the family (fused-kernel WaveNets or LSTMs); the
-    others must match it in everything but their weights -- for LSTMs: sample rate, in/out channels, num_layers,
-    input_size, hidden_size and the config object.  {ok, n_models, reason (first offending model and field), fingerprints
+    """Host-only: can these documents share a bank?  Model 0 chooses the family (fused-kernel WaveNets, general-kernel
+    WaveNets, ConvNets or LSTMs); the others must match it in everything but their weights -- for general WaveNets: every
+    array, layer, FiLM, head and condition_dsp field, hence the general kernel's descriptors (both output scales and a
+    nested condition_dsp's weights and metadata are per model); for ConvNets: channels, dilations, BatchNorm presence and
+    activation; for LSTMs: sample rate, in/out channels, num_layers, input_size, hidden_size; always the sample rate and
+    the config object.  Fused and general WaveNets do not mix (reason "model k: kernel: ...").  {ok, n_models, reason (first offending model and field), fingerprints
     (each model's state record fingerprint)}.  Needs no GPU."""
     import json
 
@@ -579,6 +587,23 @@ def bank_check(configs) -> dict:
     arr, keep = _text_array(_documents(configs))
     buf = C.create_string_buffer(1 << 16)
     rc = lib.nam_b200_bank_check_json(arr, len(keep), buf, len(buf))
+    if rc != 0:
+        _raise(rc, lib)
+    return json.loads(buf.value.decode())
+
+
+def bank_jit_prepare(configs, fast_tanh: Optional[bool] = None) -> dict:
+    """Host-only: compile (or find in the cache) the general kernel compiled for the shape of a bank of general-kernel
+    WaveNets (the kernel get_dsp_bank runs for them under jit 0 / 1 / 3).  The cache key holds no weight: every bank of one
+    shape shares the cubin.  {ok, from_cache, compile_seconds, cubin_bytes, threads, smem_bytes, why_not}.  Documents that
+    cannot share a bank, and banks of other families, raise as get_dsp_bank would.  Needs no GPU."""
+    import json
+
+    lib = _capi.load()
+    arr, keep = _text_array(_documents(configs))
+    ft = int(_using_fast_tanh if fast_tanh is None else bool(fast_tanh))
+    buf = C.create_string_buffer(1 << 16)
+    rc = lib.nam_b200_bank_jit_prepare_json(arr, len(keep), ft, buf, len(buf))
     if rc != 0:
         _raise(rc, lib)
     return json.loads(buf.value.decode())

@@ -15,12 +15,18 @@ stream, 64 streams per CTA, one pass per distinct model of a CTA).  The thread-p
 4096-frame call of 4096 such streams, so h70 runs only calls of up to --h70-max-frames frames; the others print "not
 measured".  LSTM handles are made with prewarm off (Reset's 24000-sample prewarm is not what is timed).
 
+--arch general runs wavenet_a2_max.nam reweighted per model (the general kernel; "shape": "a2_max"), --arch convnet a
+ConvNet of 8 channels, dilations 1..128 and BatchNorm ("shape": "convnet").  A general bank runs the precompiled general
+kernel with jit = 2 ("bank") and the general kernel compiled for the bank's shape with the default jit ("bank_jit", checked
+within 1e-5 of the jit = 2 bank); its "handles" arm uses the default jit (each handle compiles its own model-specialised
+kernel, so keep --handles-max-k small), and "jit" is the ordinary handle's model-specialised general kernel.
+
 Before timing, every K checks the bank's first call against fresh ordinary handles of its models at the timed sizes (up to
 --check-models models; the bank's row reports bytes_equal and max_abs_diff, and the run stops above 1e-5).  Each arm is timed over --iters calls after --warmup, the arms alternated --repeats
 times; the rate is Msamples/s (streams x frames / s) with the spread (min..max) of the repeats.  Prints the card's name and
 power limit first, then one JSON line per (K, frames, binding, arm).
 
-    python tools/bank_bench.py [--arch wavenet|lstm] [--ks 1 8 64 512] [--frames 64 4096] [--iters 10] [--warmup 2]
+    python tools/bank_bench.py [--arch wavenet|lstm|general|convnet] [--ks 1 8 64 512] [--frames 64 4096] [--iters 10] [--warmup 2]
                                [--repeats 3]
 """
 from __future__ import annotations
@@ -57,7 +63,11 @@ def family(k: int, shape: str = "a1") -> list:
                  "config": {"input_size": 1, "hidden_size": 70, "num_layers": 1},
                  "weights": [float(v) for v in np.random.default_rng(i).uniform(-0.3, 0.3, 4 * 70 * 71 + 4 * 70 + 2 * 70 + 71)]}
                 for i in range(k)]
-    base = fx.load_model({"a1": "wavenet_a1_standard", "lstm": "lstm"}[shape])
+    if shape == "convnet":
+        from tests.test_reference_build import _convnet
+
+        return [_convnet(8, [1, 2, 4, 8, 16, 32, 64, 128], True, "Tanh", i) for i in range(k)]
+    base = fx.load_model({"a1": "wavenet_a1_standard", "lstm": "lstm", "a2_max": "wavenet_a2_max"}[shape])
     w0 = np.asarray(base["weights"], np.float32)
     docs = []
     for i in range(k):
@@ -78,7 +88,7 @@ def main() -> None:
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--handles-max-k", type=int, default=64)
     ap.add_argument("--check-models", type=int, default=8)
-    ap.add_argument("--arch", choices=["wavenet", "lstm"], default="wavenet")
+    ap.add_argument("--arch", choices=["wavenet", "lstm", "general", "convnet"], default="wavenet")
     ap.add_argument("--h70-max-frames", type=int, default=64)
     args = ap.parse_args()
     os.environ.setdefault("NAM_B200_JIT_CACHE", tempfile.mkdtemp(prefix="nam_b200_jit_"))  # (the tree may be read-only)
@@ -114,7 +124,8 @@ def main() -> None:
         r0, r1 = rows
         return lambda: d.process_batch_device(x[r0].data_ptr(), y[r0].data_ptr(), r1 - r0, n_frames, F, F, cuda_stream=cs)
 
-    for shape in (["a1"] if args.arch == "wavenet" else ["lstm", "h70"]):
+    shapes = {"wavenet": ["a1"], "lstm": ["lstm", "h70"], "general": ["a2_max"], "convnet": ["convnet"]}[args.arch]
+    for shape in shapes:
         run_shape(args, shape, B, F, x, y, stream, timed, device_call)
 
 
@@ -124,7 +135,8 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
     import neuralampmodelercore_b200 as nb
 
     tag = {} if shape == "a1" else {"shape": shape}  # (the WaveNet rows keep their fields)
-    opts = {} if shape == "a1" else {"prewarm": False}
+    opts = {"prewarm": False} if shape in ("lstm", "h70") else {}
+    handle_jit = 0 if shape in ("a2_max", "convnet") else 2  # (the "handles" arm)
     singles = {}
     for jit in (2, 0):
         d = nb.get_dsp(family(1, shape)[0], batch=B, jit=jit, **opts)
@@ -135,11 +147,13 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
         docs = family(K, shape)
         bank = nb.get_dsp_bank(docs, batch=B, jit=2, **opts)
         bank.Reset(48000.0, F)
+        # a general bank with the default jit: the general kernel compiled for the bank's shape
+        bank_jit = nb.get_dsp_bank(docs, batch=B, **opts) if shape == "a2_max" else None
         per = B // K
         handles = []
         if K <= args.handles_max_k and K > 1:
             for d in docs:
-                h = nb.get_dsp(d, batch=per, jit=2, **opts)
+                h = nb.get_dsp(d, batch=per, jit=handle_jit, **opts)
                 h.Reset(48000.0, F)
                 handles.append(h)
         for binding in ("grouped", "round_robin"):
@@ -153,7 +167,7 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
                     continue
                 bank.Reset(48000.0, F)
                 bank.assign_streams(np.arange(B), models)
-                if shape != "a1":  # (an LSTM keeps h, c across Reset: every stream restarts from its model's h0 / c0)
+                if shape in ("lstm", "h70"):  # (an LSTM keeps h, c across Reset: every stream restarts from its model's h0 / c0)
                     bank.reset_streams(np.arange(B), fresh=True)
                 # correctness at the timed size: the bank's first call against fresh ordinary handles of its models
                 bank_run = device_call(bank, (0, B), n_frames)
@@ -172,9 +186,20 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
                     check["max_abs_diff"] = max(check["max_abs_diff"], float(np.max(np.abs(got[rows] - want))))
                 if check["max_abs_diff"] > 1e-5:
                     raise SystemExit(f"bank_bench: K={K} {binding} {n_frames} frames: outputs differ from the ordinary handles {check}")
-                arms = {"bank": bank_run,
+                arms = {}
+                if bank_jit is not None:
+                    bank_jit.Reset(48000.0, F)
+                    bank_jit.assign_streams(np.arange(B), models)
+                    arms["bank_jit"] = device_call(bank_jit, (0, B), n_frames)
+                    arms["bank_jit"]()
+                    stream.synchronize()
+                    check["bank_jit_state"] = bank_jit.jit_state
+                    check["bank_jit_max_abs_diff"] = float(np.max(np.abs(y[:, :n_frames].cpu().numpy() - got)))
+                    if check["bank_jit_max_abs_diff"] > 1e-5:
+                        raise SystemExit(f"bank_bench: K={K} {binding} {n_frames} frames: the default-jit bank differs {check}")
+                arms.update({"bank": bank_run,
                         "jit2": device_call(singles[2], (0, B), n_frames),
-                        "jit": device_call(singles[0], (0, B), n_frames)}
+                        "jit": device_call(singles[0], (0, B), n_frames)})
                 if handles and binding == "grouped":
                     calls = [device_call(h, (k * per, (k + 1) * per), n_frames) for k, h in enumerate(handles)]
                     arms["handles"] = lambda: [c() for c in calls]
@@ -185,7 +210,9 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
                     for a, run in arms.items():
                         ms = timed(run, args.iters)
                         rates[a].append(B * n_frames / (ms * 1e-3) / 1e6)
-                for a in ("bank", "handles", "jit2", "jit"):
+                for a in ("bank", "bank_jit", "handles", "jit2", "jit"):
+                    if a == "bank_jit" and bank_jit is None:
+                        continue
                     row = {**tag, "K": K, "frames": n_frames, "binding": binding, "arm": a}
                     if a in rates:
                         r = sorted(rates[a])
@@ -198,6 +225,8 @@ def run_shape(args, shape, B, F, x, y, stream, timed, device_call) -> None:
         for h in handles:
             h.close()
         bank.close()
+        if bank_jit is not None:
+            bank_jit.close()
     for d in singles.values():
         d.close()
 
