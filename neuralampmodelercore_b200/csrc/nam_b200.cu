@@ -678,32 +678,6 @@ constexpr WnGeometry kWnGeom[4] = {{128, 3, 8}, {256, 2, 9}, {128, 3, 6}, {256, 
 // calls of up to this many frames take the multi-stream geometry 2 / 3
 constexpr int kWnShortMaxFrames[2] = {96, 192};
 
-// (calls with a slot table run the kernel's TBL instantiation; the occupancy queries take the lower of the two, so that the
-// co-residency the tile-parallel modes rely on holds for both)
-template <int C0, int C1, int NT, int MINB, int LQ>
-void launch_wavenet_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
-{
-  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ, false, true> : wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>;
-  ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
-  kern<<<grid, NT, smem, st>>>(kp);
-  CUDA_CHECK(cudaGetLastError());
-}
-
-template <int C0, int C1, int NT, int MINB, int LQ>
-int occupancy_wavenet_variant(size_t smem)
-{
-  int best = 1 << 30;
-  for (auto kern : {wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ>, wavenet_fused_kernel<C0, C1, kWnS, NT, MINB, LQ, false, true>})
-  {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NT, smem) != cudaSuccess)
-      return 1;
-    best = std::min(best, n);
-  }
-  return best > 0 ? best : 1;
-}
-
 // lock-step tile-parallel kernels (LS = true), one stream per tile.
 //   LS geometry 0: 128 threads x 2 frames, tile 256, >= 3 CTAs/SM  (default; kernel_geometry 1)
 //   LS geometry 1: 256 threads x 2 frames, tile 512, >= 2 CTAs/SM  (kernel_geometry 2; also when tile 256 does not fit)
@@ -719,23 +693,64 @@ struct LsGeometry
 constexpr int kLsGeoms = 3;
 constexpr LsGeometry kLsGeom[kLsGeoms] = {{128, 2, 3, 8}, {256, 2, 2, 9}, {128, 1, 3, 7}};
 
-template <int C0, int C1, int S, int NT, int MINB, int LQ>
-void launch_wavenet_ls_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
+// The channel pairs the fused kernels are compiled for: (C0, C1) = the padded channels of array 0 and array 1 (0: one array)
+constexpr int kChannelPairs[][2] = {{4, 0}, {8, 0}, {16, 0}, {4, 4}, {4, 8}, {4, 16}, {8, 4}, {8, 8}, {8, 16}, {16, 4}, {16, 8}, {16, 16}};
+constexpr int kNumChannelPairs = (int)(sizeof(kChannelPairs) / sizeof(kChannelPairs[0]));
+template <int V>
+using IntC = std::integral_constant<int, V>;
+
+// f(IntC<C0>, IntC<C1>) for the listed pair (c0, c1); `kind` names the kernel in the error for a pair outside the list
+template <int P = 0, typename F>
+auto with_channel_pair(int c0, int c1, const char* kind, const F& f) -> decltype(f(IntC<4>{}, IntC<0>{}))
 {
-  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true, true> : wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>;
-  ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
-  // The tiles spin on each other's flags, so they must all be resident at once: a cooperative launch is
-  // gang-scheduled (it starts only when the whole grid fits), which keeps two such launches from different handles
-  // from starving each other.
-  void* args[] = {const_cast<void*>(static_cast<const void*>(&kp))};
-  CUDA_CHECK(cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(kern), dim3((unsigned)grid), dim3(NT), args, smem, st));
+  if constexpr (P == kNumChannelPairs)
+    throw std::runtime_error(std::string("no ") + kind + " WaveNet kernel for channel pair " + std::to_string(c0) + "/"
+                             + std::to_string(c1));
+  else
+  {
+    if (c0 == kChannelPairs[P][0] && c1 == kChannelPairs[P][1])
+      return f(IntC<kChannelPairs[P][0]>{}, IntC<kChannelPairs[P][1]>{});
+    return with_channel_pair<P + 1>(c0, c1, kind, f);
+  }
+}
+// f(IntC<g>) for g in [0, N), the last one for any g outside
+template <int N, int G = 0, typename F>
+auto with_index(int g, const F& f) -> decltype(f(IntC<0>{}))
+{
+  if constexpr (G + 1 < N)
+    if (g != G)
+      return with_index<N, G + 1>(g, f);
+  return f(IntC<G>{});
 }
 
-template <int C0, int C1, int S, int NT, int MINB, int LQ>
-int occupancy_wavenet_ls_variant(size_t smem)
+// One launch of the fused kernel; calls with a slot table run its TBL instantiation
+template <int C0, int C1, int S, int NT, int MINB, int LQ, bool LS>
+void launch_fused(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
+{
+  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, LS, true> : wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, LS>;
+  ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
+  if constexpr (LS)
+  {
+    // The tiles spin on each other's flags, so they must all be resident at once: a cooperative launch is
+    // gang-scheduled (it starts only when the whole grid fits), which keeps two such launches from different handles
+    // from starving each other.
+    void* args[] = {const_cast<void*>(static_cast<const void*>(&kp))};
+    CUDA_CHECK(cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(kern), dim3((unsigned)grid), dim3(NT), args, smem, st));
+  }
+  else
+  {
+    kern<<<grid, NT, smem, st>>>(kp);
+    CUDA_CHECK(cudaGetLastError());
+  }
+}
+
+// CTAs per SM of the fused kernel: the lower of its two instantiations, so that the co-residency the tile-parallel modes
+// rely on holds for both
+template <int C0, int C1, int S, int NT, int MINB, int LQ, bool LS>
+int occupancy_fused(size_t smem)
 {
   int best = 1 << 30;
-  for (auto kern : {wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true>, wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, true, true>})
+  for (auto kern : {wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, LS>, wavenet_fused_kernel<C0, C1, S, NT, MINB, LQ, LS, true>})
   {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     int n = 0;
@@ -746,73 +761,44 @@ int occupancy_wavenet_ls_variant(size_t smem)
   return best > 0 ? best : 1;
 }
 
-#define WN_LS_CASE(C0, C1, FN, ...)                                                                                  \
-  case (C0) * 100 + (C1):                                                                                            \
-    return geom == 0 ? FN<C0, C1, 2, 128, 3, 8>(__VA_ARGS__)                                                         \
-                     : (geom == 1 ? FN<C0, C1, 2, 256, 2, 9>(__VA_ARGS__) : FN<C0, C1, 1, 128, 3, 7>(__VA_ARGS__));
-
-#define WN_LS_DISPATCH(FN, ...)                                                                                      \
-  switch (c0 * 100 + c1)                                                                                             \
-  {                                                                                                                  \
-    WN_LS_CASE(4, 0, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(8, 0, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(16, 0, FN, __VA_ARGS__)                                                                               \
-    WN_LS_CASE(4, 4, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(4, 8, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(4, 16, FN, __VA_ARGS__)                                                                               \
-    WN_LS_CASE(8, 4, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(8, 8, FN, __VA_ARGS__)                                                                                \
-    WN_LS_CASE(8, 16, FN, __VA_ARGS__)                                                                               \
-    WN_LS_CASE(16, 4, FN, __VA_ARGS__)                                                                               \
-    WN_LS_CASE(16, 8, FN, __VA_ARGS__)                                                                               \
-    WN_LS_CASE(16, 16, FN, __VA_ARGS__)                                                                              \
-    default: throw std::runtime_error("no fused WaveNet kernel for channel pair " + std::to_string(c0) + "/"         \
-                                      + std::to_string(c1));                                                         \
-  }
-
-#define WN_CASE(C0, C1, FN, ...)                                                                                     \
-  case (C0) * 100 + (C1):                                                                                            \
-    return geom == 0 ? FN<C0, C1, 128, 3, 8>(__VA_ARGS__)                                                            \
-                     : (geom == 1 ? FN<C0, C1, 256, 2, 9>(__VA_ARGS__)                                               \
-                                  : (geom == 2 ? FN<C0, C1, 128, 3, 6>(__VA_ARGS__) : FN<C0, C1, 256, 2, 7>(__VA_ARGS__)));
-
-#define WN_DISPATCH(FN, ...)                                                                                         \
-  switch (c0 * 100 + c1)                                                                                             \
-  {                                                                                                                  \
-    WN_CASE(4, 0, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(8, 0, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(16, 0, FN, __VA_ARGS__)                                                                                  \
-    WN_CASE(4, 4, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(4, 8, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(4, 16, FN, __VA_ARGS__)                                                                                  \
-    WN_CASE(8, 4, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(8, 8, FN, __VA_ARGS__)                                                                                   \
-    WN_CASE(8, 16, FN, __VA_ARGS__)                                                                                  \
-    WN_CASE(16, 4, FN, __VA_ARGS__)                                                                                  \
-    WN_CASE(16, 8, FN, __VA_ARGS__)                                                                                  \
-    WN_CASE(16, 16, FN, __VA_ARGS__)                                                                                 \
-    default: throw std::runtime_error("no fused WaveNet kernel for channel pair " + std::to_string(c0) + "/"         \
-                                      + std::to_string(c1));                                                         \
-  }
-
 void launch_wavenet_dispatch(int c0, int c1, int geom, nam_b200_model* m, const WaveNetKernelParams& kp, int grid,
                              size_t smem, cudaStream_t st)
 {
-  WN_DISPATCH(launch_wavenet_variant, m, kp, grid, smem, st)
+  with_channel_pair(c0, c1, "fused", [&](auto C0, auto C1) {
+    with_index<4>(geom, [&](auto g) {
+      constexpr WnGeometry G = kWnGeom[decltype(g)::value];
+      launch_fused<decltype(C0)::value, decltype(C1)::value, kWnS, G.nt, G.min_ctas, G.lq, false>(m, kp, grid, smem, st);
+    });
+  });
 }
 int occupancy_wavenet_dispatch(int c0, int c1, int geom, size_t smem)
 {
-  WN_DISPATCH(occupancy_wavenet_variant, smem)
+  return with_channel_pair(c0, c1, "fused", [&](auto C0, auto C1) {
+    return with_index<4>(geom, [&](auto g) {
+      constexpr WnGeometry G = kWnGeom[decltype(g)::value];
+      return occupancy_fused<decltype(C0)::value, decltype(C1)::value, kWnS, G.nt, G.min_ctas, G.lq, false>(smem);
+    });
+  });
 }
 
 void launch_wavenet_ls_dispatch(int c0, int c1, int geom, nam_b200_model* m, const WaveNetKernelParams& kp, int grid,
                                 size_t smem, cudaStream_t st)
 {
-  WN_LS_DISPATCH(launch_wavenet_ls_variant, m, kp, grid, smem, st)
+  with_channel_pair(c0, c1, "fused", [&](auto C0, auto C1) {
+    with_index<kLsGeoms>(geom, [&](auto g) {
+      constexpr LsGeometry G = kLsGeom[decltype(g)::value];
+      launch_fused<decltype(C0)::value, decltype(C1)::value, G.s, G.nt, G.min_ctas, G.lq, true>(m, kp, grid, smem, st);
+    });
+  });
 }
 int occupancy_wavenet_ls_dispatch(int c0, int c1, int geom, size_t smem)
 {
-  WN_LS_DISPATCH(occupancy_wavenet_ls_variant, smem)
+  return with_channel_pair(c0, c1, "fused", [&](auto C0, auto C1) {
+    return with_index<kLsGeoms>(geom, [&](auto g) {
+      constexpr LsGeometry G = kLsGeom[decltype(g)::value];
+      return occupancy_fused<decltype(C0)::value, decltype(C1)::value, G.s, G.nt, G.min_ctas, G.lq, true>(smem);
+    });
+  });
 }
 
 // ---- few streams, short calls (the plugin protocol: one stream, 64-frame process() calls) ----------------------------
@@ -858,40 +844,21 @@ void launch_wavenet_lat2_variant(nam_b200_model* m, const WaveNetKernelParams& k
   }
   CUDA_CHECK(cudaGetLastError());
 }
-#define WN_LAT2_CASE(C0, C1) \
-  case (C0) * 100 + (C1): return launch_wavenet_lat2_variant<C0, C1>(m, kp, fw, smem, st);
 void launch_wavenet_lat2_dispatch(int c0, int c1, nam_b200_model* m, const WaveNetKernelParams& kp, int fw, size_t smem,
                                   cudaStream_t st)
 {
-  switch (c0 * 100 + c1)
-  {
-    WN_LAT2_CASE(4, 0) WN_LAT2_CASE(8, 0) WN_LAT2_CASE(16, 0) WN_LAT2_CASE(4, 4) WN_LAT2_CASE(4, 8) WN_LAT2_CASE(4, 16)
-    WN_LAT2_CASE(8, 4) WN_LAT2_CASE(8, 8) WN_LAT2_CASE(8, 16) WN_LAT2_CASE(16, 4) WN_LAT2_CASE(16, 8) WN_LAT2_CASE(16, 16)
-    default: throw std::runtime_error("no low-latency WaveNet kernel for channel pair " + std::to_string(c0) + "/" + std::to_string(c1));
-  }
+  with_channel_pair(c0, c1, "low-latency", [&](auto C0, auto C1) {
+    launch_wavenet_lat2_variant<decltype(C0)::value, decltype(C1)::value>(m, kp, fw, smem, st);
+  });
 }
 
 constexpr int kSmallNt = 128, kSmallLq = 7;
-template <int C0, int C1>
-void launch_wavenet_small_variant(nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem, cudaStream_t st)
-{
-  auto kern = kp.slots ? wavenet_fused_kernel<C0, C1, 1, kSmallNt, 3, kSmallLq, false, true>
-                       : wavenet_fused_kernel<C0, C1, 1, kSmallNt, 3, kSmallLq, false>;
-  ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 227 * 1024);
-  kern<<<grid, kSmallNt, smem, st>>>(kp);
-  CUDA_CHECK(cudaGetLastError());
-}
-#define WN_SMALL_CASE(C0, C1) \
-  case (C0) * 100 + (C1): return launch_wavenet_small_variant<C0, C1>(m, kp, grid, smem, st);
 void launch_wavenet_small_dispatch(int c0, int c1, nam_b200_model* m, const WaveNetKernelParams& kp, int grid, size_t smem,
                                    cudaStream_t st)
 {
-  switch (c0 * 100 + c1)
-  {
-    WN_SMALL_CASE(4, 0) WN_SMALL_CASE(8, 0) WN_SMALL_CASE(16, 0) WN_SMALL_CASE(4, 4) WN_SMALL_CASE(4, 8) WN_SMALL_CASE(4, 16)
-    WN_SMALL_CASE(8, 4) WN_SMALL_CASE(8, 8) WN_SMALL_CASE(8, 16) WN_SMALL_CASE(16, 4) WN_SMALL_CASE(16, 8) WN_SMALL_CASE(16, 16)
-    default: throw std::runtime_error("no fused WaveNet kernel for channel pair " + std::to_string(c0) + "/" + std::to_string(c1));
-  }
+  with_channel_pair(c0, c1, "fused", [&](auto C0, auto C1) {
+    launch_fused<decltype(C0)::value, decltype(C1)::value, 1, kSmallNt, 3, kSmallLq, false>(m, kp, grid, smem, st);
+  });
 }
 size_t wavenet_small_smem_bytes(const WaveNetPlan& plan)
 {
@@ -1197,12 +1164,10 @@ void launch_wavenet_spec(nam_b200_model* m, JitParams jp, cudaStream_t st)
   CUDA_CHECK(cudaLaunchKernel((const void*)m->spec_kernel, dim3(grid), dim3(m->spec_geom.nt), args, m->spec_smem, st));
 }
 
-// `slots`: the call's slot table (position b -> state row, clock), nullptr = rows stream0 + b at t_base
-void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                    long out_stride, cudaStream_t st, int stream0 = 0, const StreamRef* slots = nullptr)
+void launch_wavenet(nam_b200_model* m, const JitParams& call, cudaStream_t st)
 {
-  float* const state0 = slots ? m->d_state : m->d_state + (size_t)stream0 * (size_t)m->state_stride;
-  JitParams jp = jit_params(m, state0, d_in, d_out, in_stride, out_stride, batch, n_frames, slots);
+  JitParams jp = call;
+  const int batch = call.batch, n_frames = call.n_frames;
   if (m->use_generic && m->gen_spec_kernel != nullptr && m->opts.kernel_geometry == 0)
   {
     void* args[] = {&jp};
@@ -1216,58 +1181,58 @@ void launch_wavenet(nam_b200_model* m, const float* d_in, float* d_out, int batc
   if (m->use_generic)
   {
     GenericKernelParams gp{};
-    gp.weights = m->d_weights;
+    gp.weights = call.weights;
     gp.layers = m->d_glayers;
     gp.net = m->gplan.net;
     gp.cond = m->gplan.cond;
     gp.has_cond = m->gplan.has_cond ? 1 : 0;
-    gp.state = state0;
-    gp.slots = slots;
-    gp.state_stride = m->state_stride;
-    gp.in = d_in;
-    gp.out = d_out;
-    gp.in_stride = in_stride;
-    gp.out_stride = out_stride;
+    gp.state = call.state;
+    gp.slots = call.slots;
+    gp.state_stride = call.state_stride;
+    gp.in = call.in;
+    gp.out = call.out;
+    gp.in_stride = call.in_stride;
+    gp.out_stride = call.out_stride;
     gp.batch = batch;
     gp.n_frames = n_frames;
-    gp.t_base = m->t_base;
+    gp.t_base = call.t_base;
     // (a bank: each model's blob with its two output scales behind the weights; its calls always carry a table)
     const bool bank = m->bank_size > 1;
     gp.n_weight_floats = bank ? (int)m->weight_stride : (int)((m->n_weight_floats + 3) & ~(size_t)3);
-    gp.weight_stride = m->weight_stride;
+    gp.weight_stride = call.weight_stride;
     gp.scale_off = (int)m->gplan.weights.size();
     const size_t wbytes = (size_t)gp.n_weight_floats * sizeof(float);
     const int grid_g = std::min(batch, 16 * m->sm_count);
     if (wbytes <= 200 * 1024)
     {
       auto kern = bank ? wavenet_generic_kernel<true, true, true>
-                       : (slots ? wavenet_generic_kernel<true, true> : wavenet_generic_kernel<true>);
+                       : (call.slots ? wavenet_generic_kernel<true, true> : wavenet_generic_kernel<true>);
       ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
       kern<<<grid_g, kGenTile, wbytes, st>>>(gp);
     }
     else
       (bank ? wavenet_generic_kernel<false, true, true>
-            : (slots ? wavenet_generic_kernel<false, true> : wavenet_generic_kernel<false>))<<<grid_g, kGenTile, 0, st>>>(gp);
+            : (call.slots ? wavenet_generic_kernel<false, true> : wavenet_generic_kernel<false>))<<<grid_g, kGenTile, 0, st>>>(gp);
     CUDA_CHECK(cudaGetLastError());
     m->launches++;
     return;
   }
   const WaveNetPlan& plan = m->plan;
   WaveNetKernelParams kp{};
-  kp.weights = m->d_weights;
+  kp.weights = call.weights;
   kp.n_weight_floats = (int)plan.blob.size();
-  kp.state = state0;
-  kp.state_stride = m->state_stride;
-  kp.slots = slots;
-  kp.in = d_in;
-  kp.out = d_out;
-  kp.in_stride = in_stride;
-  kp.out_stride = out_stride;
+  kp.state = call.state;
+  kp.state_stride = call.state_stride;
+  kp.slots = call.slots;
+  kp.in = call.in;
+  kp.out = call.out;
+  kp.in_stride = call.in_stride;
+  kp.out_stride = call.out_stride;
   kp.batch = batch;
   kp.n_frames = n_frames;
-  kp.t_base = m->t_base;
+  kp.t_base = call.t_base;
   kp.head_scale = plan.head_scale;
-  kp.weight_stride = m->weight_stride;
+  kp.weight_stride = call.weight_stride;
   kp.head_scales = m->d_head_scales; // (a bank's calls always carry a table: prefix_needs_table)
   kp.n_arrays = plan.n_arrays;
   for (size_t i = 0; i < plan.arrays.size(); i++)
@@ -1486,16 +1451,13 @@ void setup_generic_bank_kernel(nam_b200_model* m)
                  + jit_loaded_note(b);
 }
 
-// `state`: rows of per-stream state to run on (nullptr = the handle's d_state; nam_b200_reset_streams prewarms a gathered
-// subset of streams in scratch rows)
-void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                 long out_stride, cudaStream_t st, float* state = nullptr, const StreamRef* slots = nullptr)
+// (call.state: the handle's d_state, or the scratch rows nam_b200_reset_streams prewarms a gathered subset of streams in)
+void launch_lstm(nam_b200_model* m, const JitParams& call, cudaStream_t st)
 {
-  if (!state)
-    state = m->d_state;
+  const int batch = call.batch;
   if (m->spec_state == 1)
   {
-    JitParams jp = jit_params(m, state, d_in, d_out, in_stride, out_stride, batch, n_frames, slots);
+    JitParams jp = call;
     void* args[] = {&jp};
     // The step rate is bound by one warp's instruction stream as long as every warp has a scheduler to itself: four
     // lanes per stream (gate-split, 8 streams per warp: a shorter dependent chain per step) while every warp still gets a
@@ -1514,27 +1476,27 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
   }
   const LstmSpec& ls = m->spec.lstm;
   LstmKernelParams kp{};
-  kp.weights = m->d_weights;
+  kp.weights = call.weights;
   kp.n_weight_floats = (int)m->n_weight_floats;
-  kp.state = state;
-  kp.state_stride = (int)m->state_stride;
-  kp.in = d_in;
-  kp.out = d_out;
-  kp.in_stride = in_stride;
-  kp.out_stride = out_stride;
+  kp.state = call.state;
+  kp.state_stride = (int)call.state_stride;
+  kp.in = call.in;
+  kp.out = call.out;
+  kp.in_stride = call.in_stride;
+  kp.out_stride = call.out_stride;
   kp.batch = batch;
-  kp.n_frames = n_frames;
+  kp.n_frames = call.n_frames;
   kp.num_layers = ls.num_layers;
   kp.input_size = ls.input_size;
   kp.hidden = ls.hidden;
   kp.fast_tanh = m->fast_tanh_runtime;
   kp.in_ch = m->spec.in_channels;
   kp.out_ch = m->spec.out_channels;
-  kp.slots = slots;
+  kp.slots = call.slots;
   // a model bank: the BANK instantiations, which read each position's model from the table (whose host copy is
   // m->h_slots[0, batch)); the kernel family is the one an ordinary handle of the same shape gets
   const bool bank = m->bank_size > 1;
-  kp.weight_stride = m->weight_stride;
+  kp.weight_stride = call.weight_stride;
   const int H = ls.hidden;
   if (H <= kLstmGroupMaxHidden && ls.num_layers <= kLstmGroupMaxLayers && kp.in_ch == 1 && kp.out_ch == 1)
   {
@@ -1630,22 +1592,23 @@ void launch_lstm(nam_b200_model* m, const float* d_in, float* d_out, int batch, 
 
 // `slots` (with m->h_slots, its host copy): each listed stream reads the buffer its history is in and the update writes the
 // other one -- no global swap, so streams left out keep theirs
-void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                   long out_stride, cudaStream_t st, const StreamRef* slots = nullptr)
+void launch_linear(nam_b200_model* m, const JitParams& call, cudaStream_t st)
 {
   const LinearSpec& li = m->spec.linear;
+  const int batch = call.batch;
+  const StreamRef* const slots = call.slots;
   LinearKernelParams kp{};
-  kp.impulse = m->d_weights;
+  kp.impulse = call.weights;
   kp.rf = li.receptive_field;
   kp.bias = li.bias_value;
-  kp.state = m->d_state;
-  kp.state_stride = (int)m->state_stride;
-  kp.in = d_in;
-  kp.out = d_out;
-  kp.in_stride = in_stride;
-  kp.out_stride = out_stride;
+  kp.state = call.state;
+  kp.state_stride = (int)call.state_stride;
+  kp.in = call.in;
+  kp.out = call.out;
+  kp.in_stride = call.in_stride;
+  kp.out_stride = call.out_stride;
   kp.batch = batch;
-  kp.n_frames = n_frames;
+  kp.n_frames = call.n_frames;
   kp.slots = slots;
   kp.state_alt = m->d_state_tmp;
   const size_t smem = (((size_t)li.receptive_field + 3) & ~(size_t)3) * 4 + ((size_t)li.receptive_field - 1 + kLinThreads) * 4;
@@ -1654,7 +1617,7 @@ void launch_linear(nam_b200_model* m, const float* d_in, float* d_out, int batch
     throw std::runtime_error("Linear receptive field too long for the direct-form kernel");
   if (batch > 65535)
     throw std::runtime_error("Linear: more than 65535 streams per call (grid.y); split the batch");
-  dim3 grid((n_frames + kLinThreads - 1) / kLinThreads, batch);
+  dim3 grid((call.n_frames + kLinThreads - 1) / kLinThreads, batch);
   linear_kernel<<<grid, kLinThreads, smem, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
@@ -1692,38 +1655,50 @@ int wavenet_chunk_streams(nam_b200_model* m)
   return 4 * per_sm * m->sm_count;
 }
 
-void launch_convnet(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride,
-                    long out_stride, cudaStream_t st, const StreamRef* slots = nullptr)
+void launch_convnet(nam_b200_model* m, const JitParams& call, cudaStream_t st)
 {
   ConvNetKernelParams kp{};
-  kp.weights = m->d_weights;
+  kp.weights = call.weights;
   kp.net = m->gplan.convnet;
-  kp.state = m->d_state;
-  kp.state_stride = m->state_stride;
-  kp.in = d_in;
-  kp.out = d_out;
-  kp.in_stride = in_stride;
-  kp.out_stride = out_stride;
-  kp.batch = batch;
-  kp.n_frames = n_frames;
-  kp.t_base = m->t_base;
+  kp.state = call.state;
+  kp.state_stride = call.state_stride;
+  kp.in = call.in;
+  kp.out = call.out;
+  kp.in_stride = call.in_stride;
+  kp.out_stride = call.out_stride;
+  kp.batch = call.batch;
+  kp.n_frames = call.n_frames;
+  kp.t_base = call.t_base;
   kp.n_weight_floats = (int)((m->n_weight_floats + 3) & ~(size_t)3);
-  kp.slots = slots;
-  kp.weight_stride = m->weight_stride; // (a bank: its calls always carry a table)
+  kp.slots = call.slots;
+  kp.weight_stride = call.weight_stride; // (a bank: its calls always carry a table)
   const bool bank = m->bank_size > 1;
   const size_t wbytes = (size_t)kp.n_weight_floats * sizeof(float);
-  const int grid = std::min(batch, 16 * m->sm_count);
+  const int grid = std::min(call.batch, 16 * m->sm_count);
   if (wbytes <= 200 * 1024)
   {
-    auto kern = bank ? convnet_kernel<true, true, true> : (slots ? convnet_kernel<true, true> : convnet_kernel<true>);
+    auto kern = bank ? convnet_kernel<true, true, true> : (call.slots ? convnet_kernel<true, true> : convnet_kernel<true>);
     ensure_max_dynamic_smem(reinterpret_cast<const void*>(kern), m->device, 200 * 1024);
     kern<<<grid, kGenTile, wbytes, st>>>(kp);
   }
   else
     (bank ? convnet_kernel<false, true, true>
-          : (slots ? convnet_kernel<false, true> : convnet_kernel<false>))<<<grid, kGenTile, 0, st>>>(kp);
+          : (call.slots ? convnet_kernel<false, true> : convnet_kernel<false>))<<<grid, kGenTile, 0, st>>>(kp);
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
+}
+
+// One call of the handle's kernel on `st`, described as jit_params() describes it
+void launch(nam_b200_model* m, const JitParams& call, cudaStream_t st)
+{
+  switch (m->spec.arch)
+  {
+    case Arch::WaveNet: return launch_wavenet(m, call, st);
+    case Arch::LSTM: return launch_lstm(m, call, st);
+    case Arch::Linear: return launch_linear(m, call, st);
+    case Arch::ConvNet: return launch_convnet(m, call, st);
+    default: throw std::runtime_error("no kernel for this architecture");
+  }
 }
 
 // ---- per-stream clocks and slot tables ----------------------------------------------------------------------------------
@@ -1773,6 +1748,12 @@ const StreamRef* push_slots(nam_b200_model* m, int n, cudaStream_t st)
   CUDA_CHECK(cudaMemcpyAsync(m->d_slots, m->h_slots.data(), (size_t)n * sizeof(StreamRef), cudaMemcpyHostToDevice, st));
   return m->d_slots;
 }
+// After the launches that read the device table: the next push_slots waits for them
+void release_slots(nam_b200_model* m, cudaStream_t st)
+{
+  CUDA_CHECK(cudaEventRecord(m->slots_free, st));
+  m->slots_used = true;
+}
 const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, int n_frames, const int32_t* counts,
                               cudaStream_t st)
 {
@@ -1792,8 +1773,7 @@ const StreamRef* upload_slots(nam_b200_model* m, const int32_t* streams, int n, 
 // by the call's n_frames (the longest count)
 void finish_table_call(nam_b200_model* m, int n, int n_frames, cudaStream_t st)
 {
-  CUDA_CHECK(cudaEventRecord(m->slots_free, st));
-  m->slots_used = true;
+  release_slots(m, st);
   m->t_base += (uint32_t)n_frames;
   for (int i = 0; i < n; i++)
     m->stream_clock[(size_t)m->h_slots[(size_t)i].stream] += (uint32_t)m->h_slots[(size_t)i].frames;
@@ -1819,14 +1799,7 @@ void run_device(nam_b200_model* m, const float* d_in, float* d_out, int batch, i
 {
   const bool table = streams != nullptr || prefix_needs_table(m, batch);
   const StreamRef* slots = table ? upload_slots(m, streams, batch, n_frames, counts, st) : nullptr;
-  switch (m->spec.arch)
-  {
-    case Arch::WaveNet: launch_wavenet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, 0, slots); break;
-    case Arch::LSTM: launch_lstm(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, nullptr, slots); break;
-    case Arch::Linear: launch_linear(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, slots); break;
-    case Arch::ConvNet: launch_convnet(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, slots); break;
-    default: throw std::runtime_error("no kernel for this architecture");
-  }
+  launch(m, jit_params(m, m->d_state, d_in, d_out, in_stride, out_stride, batch, n_frames, slots), st);
   if (table)
     finish_table_call(m, batch, n_frames, st);
   else
@@ -1943,30 +1916,45 @@ void broadcast_state(nam_b200_model* m)
   m->launches++;
 }
 
-// DSP::prewarm (dsp.cpp:67-101): zeros in max_frames blocks until >= prewarm_samples; done once on
-// stream 0 (every stream would compute the identical state) and broadcast.
-void prewarm(nam_b200_model* m)
+// DSP::prewarm's loop (dsp.cpp:67-101): zeros in max_frames blocks until >= prewarm_samples.  The staging is sized for
+// `rows` streams and the input of the first n zeroed; block(call) runs each block, `call` being n positions of zeros on
+// the handle's state rows without a table.  Nothing happens without prewarm samples.
+template <typename F>
+void prewarm_blocks(nam_b200_model* m, int n, int rows, const F& block)
 {
   const int ps = m->spec.prewarm_samples;
   if (ps <= 0)
     return;
   const int bs = std::max(m->max_frames, 1);
   const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
-  ensure_staging(m, (size_t)m->opts.max_batch * bs * std::max(ci, co));
+  ensure_staging(m, (size_t)rows * bs * std::max(ci, co));
+  CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
+  for (int done = 0; done < ps; done += bs)
+    block(jit_params(m, m->d_state, m->d_in, m->d_out, (long)(bs * ci), (long)(bs * co), n, bs, nullptr));
+}
+
+// `call` with the first n entries of m->h_slots as its table
+void launch_with_table(nam_b200_model* m, JitParams call, int n, cudaStream_t st)
+{
+  call.slots = push_slots(m, n, st);
+  launch(m, call, st);
+  release_slots(m, st);
+}
+
+// DSP::prewarm: done once on stream 0 (every stream would compute the identical state) and broadcast.
+void prewarm(nam_b200_model* m)
+{
+  if (m->spec.prewarm_samples <= 0)
+    return;
   // DSP::prewarm continues from the instance's CURRENT state (dsp.cpp:67-101).  Straight after init_state every stream
   // would compute the same thing: stream 0 runs, its state is broadcast.  Once the streams have seen different audio
   // (a standalone nam_b200_prewarm, or a Reset of an LSTM, which keeps its running state) all of them are prewarmed.
   // (a bank's streams run different models: nam_b200_reset prewarms it through prewarm_bank or prewarm_lstm_bank, a
   // standalone prewarm runs every stream with its own model)
   const bool identical = m->streams_identical && m->bank_size == 1;
-  const int nb = identical ? 1 : m->opts.max_batch;
-  CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)nb * bs * ci * sizeof(float), m->stream));
-  int done = 0;
-  while (done < ps)
-  {
-    run_device(m, m->d_in, m->d_out, nb, bs, (long)(bs * ci), (long)(bs * co), m->stream);
-    done += bs;
-  }
+  prewarm_blocks(m, identical ? 1 : m->opts.max_batch, m->opts.max_batch, [&](const JitParams& c) {
+    run_device(m, c.in, c.out, c.batch, c.n_frames, c.in_stride, c.out_stride, m->stream);
+  });
   m->streams_identical = identical; // zeros into identical streams keep them identical
   if (identical)
   {
@@ -2138,30 +2126,15 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
   }
   else
     copy_rows(m, rows, nullptr, m->d_state, d_refs, n, m->stream);
-  const int ps = m->spec.prewarm_samples;
-  if (m->opts.prewarm_on_reset && ps > 0)
-  {
-    const int bs = std::max(m->max_frames, 1);
-    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
-    ensure_staging(m, (size_t)n * bs * std::max(ci, co));
-    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
-    for (int done = 0; done < ps; done += bs)
-    {
-      const StreamRef* slots = nullptr;
-      if (m->bank_size > 1)
-      {
-        for (int i = 0; i < n; i++)
-          m->h_slots[(size_t)i] = StreamRef{i, 0u, m->stream_model[(size_t)streams[i]], bs};
-        slots = push_slots(m, n, m->stream);
-      }
-      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, rows, slots);
-      if (slots)
-      {
-        CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
-        m->slots_used = true;
-      }
-    }
-  }
+  if (m->opts.prewarm_on_reset)
+    prewarm_blocks(m, n, n, [&](JitParams call) {
+      call.state = rows;
+      if (m->bank_size == 1)
+        return launch(m, call, m->stream);
+      for (int i = 0; i < n; i++)
+        m->h_slots[(size_t)i] = StreamRef{i, 0u, m->stream_model[(size_t)streams[i]], call.n_frames};
+      launch_with_table(m, call, n, m->stream);
+    });
   copy_rows(m, m->d_state, d_refs, rows, nullptr, n, m->stream);
   mark_written(m, streams, n);
 }
@@ -2193,27 +2166,13 @@ void bank_fan_out(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t
 // takes its model's row.
 void prewarm_bank(nam_b200_model* m)
 {
-  const int ps = m->spec.prewarm_samples, K = m->bank_size;
-  const int bs = std::max(m->max_frames, 1);
-  if (ps > 0)
-  {
-    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
-    ensure_staging(m, (size_t)std::max(m->opts.max_batch, K) * bs * std::max(ci, co));
-    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)K * bs * ci * sizeof(float), m->stream));
-    for (int done = 0; done < ps; done += bs)
-    {
-      for (int k = 0; k < K; k++)
-        m->h_slots[(size_t)k] = StreamRef{m->opts.max_batch + k, m->t_base, k, bs};
-      const StreamRef* slots = push_slots(m, K, m->stream);
-      if (m->spec.arch == Arch::ConvNet)
-        launch_convnet(m, m->d_in, m->d_out, K, bs, (long)(bs * ci), (long)(bs * co), m->stream, slots);
-      else
-        launch_wavenet(m, m->d_in, m->d_out, K, bs, (long)(bs * ci), (long)(bs * co), m->stream, 0, slots);
-      CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
-      m->slots_used = true;
-      m->t_base += (uint32_t)bs;
-    }
-  }
+  const int K = m->bank_size;
+  prewarm_blocks(m, K, std::max(m->opts.max_batch, K), [&](const JitParams& call) {
+    for (int k = 0; k < K; k++)
+      m->h_slots[(size_t)k] = StreamRef{m->opts.max_batch + k, m->t_base, k, call.n_frames};
+    launch_with_table(m, call, K, m->stream);
+    m->t_base += (uint32_t)call.n_frames;
+  });
   m->fresh_clock = m->t_base;
   std::vector<int32_t> all((size_t)m->opts.max_batch);
   for (int s = 0; s < m->opts.max_batch; s++)
@@ -2260,26 +2219,133 @@ void prewarm_lstm_bank(nam_b200_model* m, bool streams)
   for (int k = 0; k < K; k++)
     models[(size_t)k] = k;
   write_lstm_initial_rows(m, m->d_state, (size_t)B, models);
-  const int ps = m->spec.prewarm_samples;
-  if (m->opts.prewarm_on_reset && ps > 0)
-  {
-    const int bs = std::max(m->max_frames, 1), n0 = streams ? B : 0, n = n0 + K;
-    const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels;
-    ensure_staging(m, (size_t)n * bs * std::max(ci, co));
-    CUDA_CHECK(cudaMemsetAsync(m->d_in, 0, (size_t)n * bs * ci * sizeof(float), m->stream));
-    for (int done = 0; done < ps; done += bs)
-    {
+  const int n0 = streams ? B : 0, n = n0 + K;
+  if (m->opts.prewarm_on_reset)
+    prewarm_blocks(m, n, n, [&](const JitParams& call) {
       for (int i = 0; i < n; i++) // streams 0 .. n0 - 1, then the model rows
-        m->h_slots[(size_t)i] = i < n0 ? StreamRef{i, m->stream_clock[(size_t)i], m->stream_model[(size_t)i], bs}
-                                       : StreamRef{B + i - n0, m->fresh_clock, i - n0, bs};
-      launch_lstm(m, m->d_in, m->d_out, n, bs, (long)(bs * ci), (long)(bs * co), m->stream, nullptr, push_slots(m, n, m->stream));
-      CUDA_CHECK(cudaEventRecord(m->slots_free, m->stream));
-      m->slots_used = true;
-    }
-  }
+        m->h_slots[(size_t)i] = i < n0 ? StreamRef{i, m->stream_clock[(size_t)i], m->stream_model[(size_t)i], call.n_frames}
+                                       : StreamRef{B + i - n0, m->fresh_clock, i - n0, call.n_frames};
+      launch_with_table(m, call, n, m->stream);
+    });
   m->rows_fast_tanh = m->fast_tanh_runtime;
   m->streams_identical = false;
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
+}
+
+// ---- which kernel serves a model ---------------------------------------------------------------------------------------
+enum class KernelFamily
+{
+  Fused, // WaveNet on the fused kernel
+  General, // WaveNet on the general kernel
+  ConvNet,
+  Lstm,
+  Linear
+};
+
+// The kernel a handle of a (non-container) model runs, and what the host prepares for it; or, when code != NAM_B200_OK,
+// create's refusal.  A refusal keeps the plans it made.
+struct KernelChoice
+{
+  int code = NAM_B200_OK;
+  std::string refusal;
+  KernelFamily family = KernelFamily::Fused;
+  WaveNetPlan plan; // WaveNet (the fused kernel's; for the general family, plan.why_not says why the fused kernel declined)
+  GenericPlan gplan; // general WaveNet, ConvNet
+  std::vector<float> blob;
+  long state_stride = 0;
+  double flops_per_frame = 0.0;
+  int variant = 0;
+};
+
+// kernel_geometry (nam_b200_options): 0 default, 1 = FFMA 128-thread, 2 = FFMA 256-thread, 3 = tensor-core (none on sm_90a),
+// 4 = the general kernel
+KernelChoice choose_kernel(const ModelSpec& s, int kernel_geometry)
+{
+  KernelChoice c;
+  auto refuse = [&](std::string why) {
+    c.code = NAM_B200_ERR_UNSUPPORTED;
+    c.refusal = std::move(why);
+    return c;
+  };
+  switch (s.arch)
+  {
+    case Arch::WaveNet:
+    {
+      WaveNetPlan& p = c.plan;
+      p = plan_wavenet(s);
+      if (p.eligible && !(s.in_channels == 1 && s.out_channels == 1))
+      {
+        p.eligible = false;
+        p.why_not = "multi-channel in / out";
+      }
+      if (p.eligible && kernel_geometry != 3 && wavenet_smem_bytes(p, kernel_geometry == 1 ? 0 : 1) > 227 * 1024)
+      {
+        // e.g. > ~50 layers of 16 channels: the general kernel keeps such weights in global memory
+        p.eligible = false;
+        p.why_not = "packed weights + tile exceed the 227 KB of shared memory of the fused kernel";
+      }
+      if (!p.eligible || kernel_geometry == 4)
+      {
+        // outside the fused families (or asked for explicitly): the general kernel
+        c.gplan = plan_generic(s);
+        if (!c.gplan.eligible)
+          return refuse("WaveNet not supported on the CUDA path: fused kernel: "
+                        + (p.eligible ? std::string("(eligible)") : p.why_not) + "; general kernel: " + c.gplan.why_not);
+        c.family = KernelFamily::General;
+        c.blob = c.gplan.weights;
+        c.state_stride = c.gplan.state_floats;
+        c.flops_per_frame = 2.0 * c.gplan.macs_per_frame;
+        c.variant = 9000;
+        return c;
+      }
+      if (kernel_geometry == 3)
+        return refuse("tensor-core WaveNet kernel: this sm_90a library has none (use kernel_geometry 0, 1, 2 or 4)");
+      c.family = KernelFamily::Fused;
+      c.blob = p.blob;
+      c.state_stride = p.state_floats;
+      c.flops_per_frame = 2.0 * p.macs_per_frame;
+      c.variant = p.cp[0] * 100 + (p.n_arrays > 1 ? p.cp[1] : 0);
+      return c;
+    }
+    case Arch::LSTM:
+    {
+      const LstmSpec& ls = s.lstm;
+      const std::string why = lstm_refusal(s);
+      if (!why.empty())
+        return refuse(why);
+      double macs = 0.0;
+      for (const auto& cell : ls.cells)
+        macs += 4.0 * cell.hidden * (cell.input_size + cell.hidden);
+      macs += (double)ls.hidden * s.out_channels;
+      c.family = KernelFamily::Lstm;
+      c.blob = lstm_blob(s);
+      c.state_stride = ((long)ls.num_layers * 2 * ls.hidden + 3) & ~3L;
+      c.flops_per_frame = 2.0 * macs;
+      c.variant = 2000 + ls.hidden;
+      return c;
+    }
+    case Arch::Linear:
+      if (!(s.in_channels == 1 && s.out_channels == 1))
+        return refuse("Linear on the CUDA path is mono in / mono out (model has " + std::to_string(s.in_channels) + " in, "
+                      + std::to_string(s.out_channels) + " out channels)");
+      c.family = KernelFamily::Linear;
+      c.blob = s.linear.impulse;
+      c.state_stride = ((long)std::max(s.linear.receptive_field - 1, 1) + 3) & ~3L;
+      c.flops_per_frame = 2.0 * s.linear.receptive_field;
+      c.variant = 3000;
+      return c;
+    case Arch::ConvNet:
+      c.gplan = plan_convnet(s);
+      if (!c.gplan.eligible)
+        return refuse("ConvNet not supported on the CUDA path: " + c.gplan.why_not);
+      c.family = KernelFamily::ConvNet;
+      c.blob = c.gplan.weights;
+      c.state_stride = std::max(c.gplan.state_floats, 4L);
+      c.flops_per_frame = 2.0 * c.gplan.macs_per_frame;
+      c.variant = 9500;
+      return c;
+    default: return refuse("no CUDA kernel for architecture " + s.architecture);
+  }
 }
 
 int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_model** out)
@@ -2348,101 +2414,31 @@ int create_common(ModelSpec&& spec, const nam_b200_options* user_opts, nam_b200_
     CUDA_CHECK(cudaEventCreate(&m->ev0));
     CUDA_CHECK(cudaEventCreate(&m->ev1));
 
-    // multi-channel models: WaveNet through the general kernel, LSTM through the thread-per-stream kernel
-    const bool mono = m->spec.in_channels == 1 && m->spec.out_channels == 1;
-    if (!mono && m->spec.arch == Arch::Linear)
-      return fail(NAM_B200_ERR_UNSUPPORTED, "Linear on the CUDA path is mono in / mono out (model has "
-                                              + std::to_string(m->spec.in_channels) + " in, "
-                                              + std::to_string(m->spec.out_channels) + " out channels)");
-    std::vector<float> blob;
-    switch (m->spec.arch)
+    KernelChoice c = choose_kernel(m->spec, m->opts.kernel_geometry);
+    if (c.code != NAM_B200_OK)
+      return fail(c.code, c.refusal);
+    m->plan = std::move(c.plan);
+    m->gplan = std::move(c.gplan);
+    m->use_generic = c.family == KernelFamily::General;
+    m->state_stride = c.state_stride;
+    m->flops_per_frame = c.flops_per_frame;
+    m->variant = c.variant;
+    switch (c.family)
     {
-      case Arch::WaveNet:
-      {
-        m->plan = plan_wavenet(m->spec);
-        if (!mono && m->plan.eligible)
-        {
-          m->plan.eligible = false;
-          m->plan.why_not = "multi-channel in / out";
-        }
-        if (m->plan.eligible && m->opts.kernel_geometry != 3
-            && wavenet_smem_bytes(m->plan, m->opts.kernel_geometry == 1 ? 0 : 1) > 227 * 1024)
-        {
-          // e.g. > ~50 layers of 16 channels: the general kernel keeps such weights in global memory
-          m->plan.eligible = false;
-          m->plan.why_not = "packed weights + tile exceed the 227 KB of shared memory of the fused kernel";
-        }
-        if (!m->plan.eligible || m->opts.kernel_geometry == 4)
-        {
-          // outside the fused families (or asked for explicitly): the general kernel
-          m->gplan = plan_generic(m->spec);
-          if (!m->gplan.eligible)
-            return fail(NAM_B200_ERR_UNSUPPORTED,
-                        "WaveNet not supported on the CUDA path: fused kernel: "
-                          + (m->plan.eligible ? std::string("(eligible)") : m->plan.why_not) + "; general kernel: " + m->gplan.why_not);
-          m->use_generic = true;
-          setup_generic_spec_kernel(m.get()); // throws when jit = 1 and the specialised general kernel cannot be had
-          blob = m->gplan.weights;
-          m->state_stride = m->gplan.state_floats;
-          m->flops_per_frame = 2.0 * m->gplan.macs_per_frame;
-          m->variant = 9000;
-          CUDA_CHECK(cudaMalloc(&m->d_glayers, std::max<size_t>(m->gplan.layers.size(), 1) * sizeof(GLayer)));
-          CUDA_CHECK(cudaMemcpy(m->d_glayers, m->gplan.layers.data(), m->gplan.layers.size() * sizeof(GLayer),
-                                cudaMemcpyHostToDevice));
-          break;
-        }
-        blob = m->plan.blob;
-        m->state_stride = m->plan.state_floats;
-        m->flops_per_frame = 2.0 * m->plan.macs_per_frame;
-        m->variant = m->plan.cp[0] * 100 + (m->plan.n_arrays > 1 ? m->plan.cp[1] : 0);
-        // option: 0 default, 1 = FFMA 128-thread, 2 = FFMA 256-thread, 3 = tensor-core (none on sm_90a)
-        if (m->opts.kernel_geometry == 3)
-          return fail(NAM_B200_ERR_UNSUPPORTED, "tensor-core WaveNet kernel: this sm_90a library has none (use kernel_geometry "
-                                                "0, 1, 2 or 4)");
+      case KernelFamily::General:
+        setup_generic_spec_kernel(m.get()); // throws when jit = 1 and the specialised general kernel cannot be had
+        CUDA_CHECK(cudaMalloc(&m->d_glayers, std::max<size_t>(m->gplan.layers.size(), 1) * sizeof(GLayer)));
+        CUDA_CHECK(cudaMemcpy(m->d_glayers, m->gplan.layers.data(), m->gplan.layers.size() * sizeof(GLayer),
+                              cudaMemcpyHostToDevice));
+        break;
+      case KernelFamily::Fused:
         m->wn_geometry = (m->opts.kernel_geometry == 1) ? 0 : 1;
-        if (wavenet_smem_bytes(m->plan, m->wn_geometry) > 227 * 1024)
-          return fail(NAM_B200_ERR_UNSUPPORTED, "WaveNet weights do not fit in shared memory");
         setup_spec_kernel(m.get());
         break;
-      }
-      case Arch::LSTM:
-      {
-        const LstmSpec& ls = m->spec.lstm;
-        const std::string why = lstm_refusal(m->spec);
-        if (!why.empty())
-          return fail(NAM_B200_ERR_UNSUPPORTED, why);
-        double macs = 0.0;
-        for (const auto& c : ls.cells)
-          macs += 4.0 * c.hidden * (c.input_size + c.hidden);
-        blob = lstm_blob(m->spec);
-        macs += (double)ls.hidden * m->spec.out_channels;
-        m->state_stride = ((long)ls.num_layers * 2 * ls.hidden + 3) & ~3L;
-        m->flops_per_frame = 2.0 * macs;
-        m->variant = 2000 + ls.hidden;
-        setup_lstm_spec_kernel(m.get());
-        break;
-      }
-      case Arch::Linear:
-      {
-        blob = m->spec.linear.impulse;
-        m->state_stride = ((long)std::max(m->spec.linear.receptive_field - 1, 1) + 3) & ~3L;
-        m->flops_per_frame = 2.0 * m->spec.linear.receptive_field;
-        m->variant = 3000;
-        break;
-      }
-      case Arch::ConvNet:
-      {
-        m->gplan = plan_convnet(m->spec);
-        if (!m->gplan.eligible)
-          return fail(NAM_B200_ERR_UNSUPPORTED, "ConvNet not supported on the CUDA path: " + m->gplan.why_not);
-        blob = m->gplan.weights;
-        m->state_stride = std::max(m->gplan.state_floats, 4L);
-        m->flops_per_frame = 2.0 * m->gplan.macs_per_frame;
-        m->variant = 9500;
-        break;
-      }
-      default: return fail(NAM_B200_ERR_UNSUPPORTED, "no CUDA kernel for architecture " + m->spec.architecture);
+      case KernelFamily::Lstm: setup_lstm_spec_kernel(m.get()); break;
+      default: break;
     }
+    std::vector<float> blob = std::move(c.blob);
     m->n_weight_floats = blob.size();
     const size_t alloc_floats = (blob.size() + 3) & ~(size_t)3;
     blob.resize(alloc_floats, 0.0f);
@@ -2730,7 +2726,9 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
       CUDA_CHECK(cudaStreamWaitEvent(m->stream, e_in, 0));
       if (padded)
         CUDA_CHECK(cudaMemsetAsync(dout, 0, (size_t)nb * row, m->stream));
-      launch_wavenet(m, din, dout, nb, n_frames, n_frames, n_frames, m->stream, s0, slots ? slots + s0 : nullptr);
+      // (without a table, the chunk's positions are state rows s0 ..)
+      float* const state = slots ? m->d_state : m->d_state + (size_t)s0 * (size_t)m->state_stride;
+      launch(m, jit_params(m, state, din, dout, n_frames, n_frames, nb, n_frames, slots ? slots + s0 : nullptr), m->stream);
       CUDA_CHECK(cudaEventRecord(e_k, m->stream));
       CUDA_CHECK(cudaStreamWaitEvent(m->copy_out, e_k, 0));
       CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s0 * out_stride, (size_t)out_stride * sizeof(float), dout, row, row,
@@ -2824,19 +2822,11 @@ constexpr size_t kRecordStagingBytes = (size_t)64 << 20;
 // WaveNet's head_scale, the last weight, and an LSTM's h0 / c0 and head included): the same expected sample rate (as
 // ContainerModel requires of its sub-models), the same config object, and the same packed form apart from the blob's values
 // (WaveNetPlan, GenericPlan) or, for an LSTM, the same channels, layers and sizes.
-enum class BankFamily
-{
-  Fused,
-  General,
-  ConvNet,
-  Lstm
-};
-
 struct BankCheck
 {
   int code = NAM_B200_OK;
   std::string reason; // names the first offending model and the field
-  BankFamily family = BankFamily::Fused;
+  KernelFamily family = KernelFamily::Fused;
   std::vector<WaveNetPlan> plans; // fused family
   std::vector<GenericPlan> gplans; // general WaveNets and ConvNets
 };
@@ -3105,7 +3095,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     return refuse(NAM_B200_ERR_INVALID_ARGUMENT, "n_models must be >= 1");
   if (specs[0].arch == Arch::LSTM)
   {
-    r.family = BankFamily::Lstm;
+    r.family = KernelFamily::Lstm;
     for (size_t k = 0; k < specs.size(); k++)
     {
       const std::string mk = "model " + std::to_string(k) + ": ";
@@ -3124,7 +3114,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     }
     return r;
   }
-  auto family_name = [](BankFamily f) { return f == BankFamily::Fused ? "fused" : "general"; };
+  auto family_name = [](KernelFamily f) { return f == KernelFamily::Fused ? "fused" : "general"; };
   for (size_t k = 0; k < specs.size(); k++)
   {
     const ModelSpec& s = specs[k];
@@ -3138,54 +3128,25 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     if (s.arch != specs[0].arch)
       return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + s.architecture
                                                 + ": a bank's models share model 0's architecture (" + specs[0].architecture + ")");
-    if (s.arch == Arch::ConvNet)
-    {
-      // (what an ordinary handle of the model would refuse)
-      GenericPlan gp = plan_convnet(s);
-      if (!gp.eligible)
-        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "ConvNet not supported on the CUDA path: " + gp.why_not);
-      r.family = BankFamily::ConvNet;
-      r.gplans.push_back(std::move(gp));
-      continue;
-    }
-    // the kernel an ordinary handle of the model gets by default (create_common): the fused one when the model is eligible,
-    // mono and fits its shared memory, else the general one
-    WaveNetPlan plan = plan_wavenet(s);
-    if (plan.eligible && !(s.in_channels == 1 && s.out_channels == 1))
-    {
-      plan.eligible = false;
-      plan.why_not = "multi-channel in / out";
-    }
-    if (plan.eligible && wavenet_smem_bytes(plan, 1) > 227 * 1024)
-    {
-      plan.eligible = false;
-      plan.why_not = "packed weights + tile exceed the shared memory of the fused kernel";
-    }
-    BankFamily f = BankFamily::Fused;
-    GenericPlan gp;
-    if (!plan.eligible)
-    {
-      gp = plan_generic(s);
-      if (!gp.eligible)
-        return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "kernel: WaveNet not supported on the CUDA path: fused kernel: "
-                                                  + plan.why_not + "; general kernel: " + gp.why_not);
-      f = BankFamily::General;
-    }
+    // the kernel an ordinary handle of the model gets by default, or its refusal
+    KernelChoice c = choose_kernel(s, 0);
+    if (c.code != NAM_B200_OK)
+      return refuse(c.code, mk + (s.arch == Arch::WaveNet ? "kernel: " : "") + c.refusal);
     if (k == 0)
-      r.family = f;
-    else if (f != r.family)
+      r.family = c.family;
+    else if (c.family != r.family)
       return refuse(NAM_B200_ERR_UNSUPPORTED,
-                    mk + "kernel: served by the " + family_name(f) + " kernel"
-                      + (f == BankFamily::General ? " (fused kernel: " + plan.why_not + ")" : std::string())
+                    mk + "kernel: served by the " + family_name(c.family) + " kernel"
+                      + (c.family == KernelFamily::General ? " (fused kernel: " + c.plan.why_not + ")" : std::string())
                       + "; model 0 (" + family_name(r.family) + " family) chooses the bank's kernel family");
-    if (f == BankFamily::Fused)
-      r.plans.push_back(std::move(plan));
+    if (c.family == KernelFamily::Fused)
+      r.plans.push_back(std::move(c.plan));
     else
-      r.gplans.push_back(std::move(gp));
+      r.gplans.push_back(std::move(c.gplan));
   }
   for (size_t k = 1; k < specs.size(); k++)
   {
-    const std::string d = r.family == BankFamily::Fused
+    const std::string d = r.family == KernelFamily::Fused
                             ? bank_difference((int)k, specs[k], r.plans[k], specs[0], r.plans[0])
                             : general_bank_difference((int)k, specs[k], r.gplans[k], specs[0], r.gplans[0]);
     if (!d.empty())
@@ -3199,7 +3160,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
 void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const BankCheck& bc)
 {
   const int K = (int)specs.size();
-  const bool lstm = bc.family == BankFamily::Lstm, fused = bc.family == BankFamily::Fused;
+  const bool lstm = bc.family == KernelFamily::Lstm, fused = bc.family == KernelFamily::Fused;
   m->bank_size = K;
   // model k's blob: the fused family's packed blob (its output scale goes to d_head_scales), an LSTM's weights, or the
   // general kernel's weights -- a general WaveNet's followed by its net and condition_dsp output scales, which the BANK
@@ -3256,7 +3217,7 @@ void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const BankChe
   m->spec_state = 0;
   m->spec_note = "model bank of " + std::to_string(K) + " models: the precompiled kernels, which read each stream's weights as "
                  "data (a model-specialised kernel compiles one model's weights into its code)";
-  if (bc.family == BankFamily::General)
+  if (bc.family == KernelFamily::General)
     setup_generic_bank_kernel(m); // (throws under jit = 1 when the shape-compiled kernel cannot be had)
   init_state(m);
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -3274,26 +3235,26 @@ int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opt
     std::memcpy(&o, user_opts, std::min<size_t>(sizeof o, (size_t)std::max(user_opts->struct_size, 0)));
     o.struct_size = sizeof o;
   }
-  if (o.jit == 1 && (bc.family == BankFamily::Fused || bc.family == BankFamily::Lstm))
+  if (o.jit == 1 && (bc.family == KernelFamily::Fused || bc.family == KernelFamily::Lstm))
     return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: jit = 1 (required) cannot be met: a model-specialised kernel compiles "
                                           "one model's weights into its code, a bank's streams each bring their own");
-  if (o.kernel_geometry == 4 && (bc.family == BankFamily::Fused || bc.family == BankFamily::Lstm))
+  if (o.kernel_geometry == 4 && (bc.family == KernelFamily::Fused || bc.family == KernelFamily::Lstm))
     return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: kernel_geometry 4 (the general kernel) does not take banks of the fused "
                                           "WaveNet or LSTM families (model 0 chooses the family)");
   // Fused and LSTM banks: jit 0 / 3 run the precompiled kernels, silently (nam_b200_jit_note says why).  General banks: model
   // 0's handle is made without its model-specialised kernel, then setup_bank applies the requested jit to the kernel compiled
   // for the bank's shape.  ConvNet banks take jit as an ordinary ConvNet handle does (it has no compiled kernel).
   const int user_jit = o.jit;
-  if (bc.family != BankFamily::ConvNet)
+  if (bc.family != KernelFamily::ConvNet)
     o.jit = 2;
-  if (bc.family == BankFamily::General && o.kernel_geometry != 0)
+  if (bc.family == KernelFamily::General && o.kernel_geometry != 0)
     o.kernel_geometry = 4; // (the general kernel is the family's: a fused geometry must not move model 0 onto the fused kernel)
   nam_b200_model* h = nullptr;
   const int rc = create_common(ModelSpec(specs[0]), &o, &h);
   if (rc != NAM_B200_OK)
     return rc;
   std::unique_ptr<nam_b200_model> m(h);
-  if (bc.family == BankFamily::General)
+  if (bc.family == KernelFamily::General)
     m->opts.jit = user_jit;
   const int rc2 = guarded(m.get(), [&]() -> int {
     setup_bank(m.get(), std::move(specs), bc);
@@ -3387,10 +3348,6 @@ static int inspect_spec(const ModelSpec& spec, char* out, int64_t capacity)
 {
   if (!out || capacity <= 0)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null output buffer");
-  std::string kernel = "unsupported", reason;
-  double flops = 0.0;
-  long state_floats = 0;
-  int variant = 0;
   if (spec.arch == Arch::Container)
   {
     // describe the default (largest) sub-model; the container itself only dispatches
@@ -3406,74 +3363,12 @@ static int inspect_spec(const ModelSpec& spec, char* out, int64_t capacity)
     std::snprintf(out, (size_t)capacity, "%s", text.c_str());
     return NAM_B200_OK;
   }
-  const bool mono = spec.in_channels == 1 && spec.out_channels == 1;
-  if (!mono && spec.arch == Arch::Linear)
-    reason = "Linear on the CUDA path is mono in / mono out";
-  else if (spec.arch == Arch::WaveNet)
-  {
-    WaveNetPlan plan = plan_wavenet(spec);
-    if (!mono && plan.eligible)
-    {
-      plan.eligible = false;
-      plan.why_not = "multi-channel in / out";
-    }
-    if (plan.eligible)
-    {
-      kernel = "fused";
-      flops = 2.0 * plan.macs_per_frame;
-      state_floats = plan.state_floats;
-      variant = plan.cp[0] * 100 + (plan.n_arrays > 1 ? plan.cp[1] : 0);
-    }
-    else
-    {
-      const GenericPlan gp = plan_generic(spec);
-      if (gp.eligible)
-      {
-        kernel = "generic";
-        flops = 2.0 * gp.macs_per_frame;
-        state_floats = gp.state_floats;
-        variant = 9000;
-        reason = "fused kernel: " + plan.why_not;
-      }
-      else
-        reason = plan.why_not + "; general kernel: " + gp.why_not;
-    }
-  }
-  else if (spec.arch == Arch::LSTM)
-  {
-    if (spec.lstm.input_size != spec.in_channels || spec.lstm.num_layers < 1)
-      reason = "LSTM input_size != in_channels or no layers";
-    else
-    {
-      kernel = "lstm";
-      double macs = (double)spec.lstm.hidden * spec.out_channels;
-      for (const auto& c : spec.lstm.cells)
-        macs += 4.0 * c.hidden * (c.input_size + c.hidden);
-      flops = 2.0 * macs;
-      state_floats = (long)spec.lstm.num_layers * 2 * spec.lstm.hidden;
-      variant = 2000 + spec.lstm.hidden;
-    }
-  }
-  else if (spec.arch == Arch::ConvNet)
-  {
-    const GenericPlan gp = plan_convnet(spec);
-    if (gp.eligible)
-    {
-      kernel = "convnet";
-      flops = 2.0 * gp.macs_per_frame;
-      state_floats = gp.state_floats;
-      variant = 9500;
-    }
-    else
-      reason = gp.why_not;
-  }
-  else
-  {
-    kernel = "linear";
-    flops = 2.0 * spec.linear.receptive_field;
-    state_floats = std::max(spec.linear.receptive_field - 1, 0);
-    variant = 3000;
-  }
+  // what a handle with the default options runs
+  const KernelChoice c = choose_kernel(spec, 0);
+  static const char* const kernel_names[] = {"fused", "generic", "convnet", "lstm", "linear"};
+  const bool ok = c.code == NAM_B200_OK;
+  const char* kernel = ok ? kernel_names[(int)c.family] : "unsupported";
+  std::string reason = !ok ? c.refusal : (c.family == KernelFamily::General ? "fused kernel: " + c.plan.why_not : "");
   for (auto& ch : reason)
     if (ch == '"' || ch == '\\' || ch == '\n')
       ch = ' ';
@@ -3484,7 +3379,7 @@ static int inspect_spec(const ModelSpec& spec, char* out, int64_t capacity)
                 "\"state_bytes_per_stream\": %ld, \"kernel\": \"%s\", \"kernel_variant\": %d, \"has_loudness\": %s, "
                 "\"loudness\": %.17g, \"reason\": \"%s\"}",
                 spec.architecture.c_str(), spec.in_channels, spec.out_channels, spec.prewarm_samples, spec.n_weights,
-                spec.sample_rate, flops, state_floats * 4, kernel.c_str(), variant, spec.loudness ? "true" : "false",
+                spec.sample_rate, c.flops_per_frame, c.state_stride * 4, kernel, c.variant, spec.loudness ? "true" : "false",
                 spec.loudness.value_or(0.0), reason.c_str());
   std::snprintf(out, (size_t)capacity, "%s", buf);
   return NAM_B200_OK;
@@ -3526,21 +3421,16 @@ int nam_b200_jit_prepare_json_for_batch(const char* nam_json_text, int fast_tanh
     const ModelSpec ms = model_spec_from_text(nam_json_text, lo);
     if (ms.arch != Arch::WaveNet && ms.arch != Arch::LSTM)
       return fail(NAM_B200_ERR_UNSUPPORTED, "only WaveNets and LSTMs have model-specialised kernels");
-    SpecBuild b;
-    bool fused_family = false;
-    if (ms.arch == Arch::LSTM)
-      b = build_lstm_spec_kernel(ms);
-    else
-    {
-      const WaveNetPlan wp = plan_wavenet(ms);
-      fused_family = wp.eligible && ms.in_channels == 1 && ms.out_channels == 1;
-      b = fused_family ? build_spec_kernel(wp, spec_geometry_for(std::max(max_batch, 1), 132))  // H100 SXM
-                       : build_generic_spec_kernel(plan_generic(ms)); // every other WaveNet: the general kernel, compiled
-    }
+    // the kernel a handle with the default options looks for (a WaveNet create refuses: its general kernel's refusal)
+    const KernelChoice c = choose_kernel(ms, 0);
+    const bool fused_family = ms.arch == Arch::WaveNet && c.code == NAM_B200_OK && c.family == KernelFamily::Fused;
+    SpecBuild b = ms.arch == Arch::LSTM ? build_lstm_spec_kernel(ms)
+                  : fused_family        ? build_spec_kernel(c.plan, spec_geometry_for(std::max(max_batch, 1), 132)) // H100 SXM
+                                        : build_generic_spec_kernel(c.gplan);
     // WaveNets: also the low-latency kernel for 64-frame calls (the plugin protocol), so that a first Reset finds it cached
     SpecBuild lat;
-    if (ms.arch == Arch::WaveNet && fused_family)
-      lat = build_lat_kernel(plan_wavenet(ms), 2);
+    if (fused_family)
+      lat = build_lat_kernel(c.plan, 2);
     std::string why;
     for (char c : b.why_not.substr(0, 600))
       why += (c == '"' || c == '\\') ? '\'' : (c == '\n' ? ' ' : c);
@@ -4091,7 +3981,7 @@ int nam_b200_bank_jit_prepare_json(const char* const* texts, int n_models, int f
   const BankCheck bc = check_bank(specs);
   if (bc.code != NAM_B200_OK)
     return fail(bc.code, "model bank: " + bc.reason);
-  if (bc.family != BankFamily::General)
+  if (bc.family != KernelFamily::General)
     return fail(NAM_B200_ERR_UNSUPPORTED, "model bank: only banks of general-kernel WaveNets have a shape-compiled kernel");
   const SpecBuild b = build_generic_spec_kernel(bc.gplans[0], true);
   std::string why;
