@@ -158,8 +158,16 @@ struct Packer
       G.head_size = A.head_size;
       G.layer0 = (int)plan.layers.size();
       G.n_layers = (int)A.layers.size();
+      // the config's widths, named as the config names them (the matrices below would only say "matrix output width")
+      width(A.channels, "channels");
       width(A.condition_size, "condition size");
       width(A.head_size, "head size");
+      for (const LayerSpec& L : A.layers)
+      {
+        width(L.conv.out, L.gating == Gating::None ? "bottleneck" : "2 x bottleneck (gated / blended layer)");
+        if (L.has_h1x1)
+          width(L.h1x1.out, "head1x1 out_channels");
+      }
       if (a > 0 && wn.arrays[a - 1].head_size != A.head_out_size() && err.empty())
         err = "head size of array " + std::to_string(a - 1) + " does not feed array " + std::to_string(a);
       G.rechannel = mat(A.rechannel);
@@ -191,7 +199,8 @@ struct Packer
     {
       if ((int)wn.post_head.convs.size() > kGenMaxHeadConvs)
       {
-        err = "post-stack head with " + std::to_string(wn.post_head.convs.size()) + " convolutions";
+        err = "post-stack head with " + std::to_string(wn.post_head.convs.size()) + " convolutions (general kernel handles up to "
+              + std::to_string(kGenMaxHeadConvs) + ")";
         return false;
       }
       N.n_head_convs = (int)wn.post_head.convs.size();
