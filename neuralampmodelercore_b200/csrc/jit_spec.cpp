@@ -361,10 +361,35 @@ std::string spec_header_source(const WaveNetPlan& plan)
   return o.str();
 }
 
-SpecBuild build_spec_kernel(const WaveNetPlan& plan, const SpecGeometry& g)
+void spec_tile_geometry(const WaveNetPlan& plan, SpecGeometry& g)
+{
+  // FFMAs per thread and frame between two barriers: per history unit (a layer, or a convolutional head)
+  long ffma = 0;
+  int units = 0;
+  for (int a = 0; a < plan.n_arrays; a++)
+  {
+    const ArrayDesc& A = plan.arrays[a];
+    const long c = plan.cp[a], hout = a + 1 == plan.n_arrays ? 1 : plan.cp[a + 1];
+    for (int i = 0; i < A.n_layers; i++, units++)
+      ffma += (plan.layers[A.layer0 + i].kernel + 1) * c * c; // dilated convolution + 1x1
+    if (A.head_kernel > 1)
+      ffma += A.head_kernel * c * hout, units++;
+  }
+  int pmax = 0;
+  for (int a = 0; a < plan.n_arrays; a++)
+    pmax = std::max(pmax, plan.cp[a] / 4);
+  const bool fits = (size_t)pmax * (size_t)(plan.max_lookback + 1024) * 16 <= 226u * 1024u;
+  const bool wide = fits && units > 0 && ffma >= 512L * units;
+  g.nt = wide ? 1024 : 512;
+  g.min_ctas = wide ? 1 : 2;
+}
+
+SpecBuild build_spec_kernel(const WaveNetPlan& plan, const SpecGeometry& requested)
 {
   SpecBuild r;
-  r.geom = g;
+  r.geom = requested;
+  spec_tile_geometry(plan, r.geom);
+  const SpecGeometry& g = r.geom;
   if (!spec_eligible(plan, g, &r.why_not))
     return r;
   r.staged_cols = plan.max_lookback;

@@ -18,7 +18,7 @@ namespace namb200
 
 struct SpecGeometry
 {
-  int nt = 512; // threads per CTA == frames per tile (one frame per thread)
+  int nt = 512; // threads per CTA == frames per tile (one frame per thread); build_spec_kernel: spec_tile_geometry
   int min_ctas = 2; // __launch_bounds__ second argument
   int short_streams = 8; // streams per CTA of the short-call entry point (64 frames each)
   int short128_streams = 4, short256_streams = 2; // ... of the entry points for calls of up to 128 / 256 frames
@@ -38,6 +38,15 @@ struct SpecBuild
   double compile_seconds = 0.0;
   size_t smem_bytes() const { return (size_t)max_planes * (size_t)(staged_cols + geom.nt) * 16; }
 };
+
+/// The throughput kernel's tile for `plan` (g.nt, g.min_ctas): one 1024-thread CTA per SM when its history window and
+/// tile fit in shared memory and the model does at least 512 FFMAs per thread and frame per history unit (layer or
+/// convolutional head), else two 512-thread CTAs per SM.  A tile stages its stream's whole ring set and writes back its
+/// newest columns, so 1024-frame tiles halve that traffic per frame, and one resident stream per SM keeps the resident
+/// rings in half of L2 where two 512-thread CTAs per SM filled it.  But a single CTA per SM has no second CTA to fill its
+/// barrier drains, so a model needs enough work between two barriers to come out ahead (H100: a1_standard, 640 FFMAs per
+/// unit, +70%; a2_full, 483, -15%; DESIGN.md 2.1b).  Any model that fits two 512-thread CTAs per SM fits one of 1024.
+void spec_tile_geometry(const WaveNetPlan& plan, SpecGeometry& g);
 
 /// Can wavenet_spec.cuh serve this plan?  (The plan must already be eligible for the generic fused kernel.)
 bool spec_eligible(const WaveNetPlan& plan, const SpecGeometry& g, std::string* why_not);

@@ -983,9 +983,9 @@ size_t wavenet_smem_bytes(const WaveNetPlan& plan, int geom)
 // ---- tensor-core variant dispatch ---------------------------------------------------------------
 // `stream0`: index of the handle's stream that d_in / d_out row 0 belongs to (chunked host calls)
 // ---- model-specialised kernel (wavenet_spec.cuh, compiled per model by jit_spec.cpp) ----------------------------------
-// Geometry of the specialised kernel for a handle of `max_batch` streams.  Streams per CTA of the short-call entry point:
-// the count that fills whole waves of 2 CTAs per SM best (4096 streams on 132 SMs: 8 per CTA = 512 CTAs = 1.94 waves, 7 per
-// CTA = 586 = 2.22 waves).
+// Geometry of the specialised kernel for a handle of `max_batch` streams (its tile is the model's: spec_tile_geometry).
+// Streams per CTA of the short-call entry point: the count that fills whole waves of 2 CTAs per SM best (4096 streams on
+// 132 SMs: 8 per CTA = 512 CTAs = 1.94 waves, 7 per CTA = 586 = 2.22 waves).
 SpecGeometry spec_geometry_for(int max_batch, int sm_count)
 {
   SpecGeometry g;

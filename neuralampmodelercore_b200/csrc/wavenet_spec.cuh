@@ -16,7 +16,12 @@
 //   ascending), so its results are bit-identical to the generic fused kernel's.
 //
 // Mapping: one persistent CTA owns one stream at a time and walks its call in tiles of T = NT frames; thread t owns
-// frames {t, t + NT, ..} for the whole depth of the network (see wavenet_fused.cuh).  What is new here:
+// frames {t, t + NT, ..} for the whole depth of the network (see wavenet_fused.cuh).  NT = 1024 on one CTA per SM, or 512
+// on two (spec_tile_geometry, jit_spec.h): every tile stages its stream's whole ring set and writes its newest columns
+// back, so that traffic per frame falls with the tile length, and one resident stream per SM keeps the resident rings in
+// half of L2 (a1_standard: 383 B of ring traffic per frame and 25.9 MB of resident rings, against 671 B and 51.9 MB --
+// all of H100's L2 -- with two 512-thread CTAs per SM; DESIGN.md 2.1b).  The call's input and output are read and written
+// once, with an L2 evict-first policy, so that they do not push the rings out.  What is new here:
 //   * TMA-engine staging of the history (cp.async.bulk, SASS UBLKCP): before a layer runs, the last `lookback` columns of
 //     its input ring are copied global -> shared by bulk-async copies that complete on an mbarrier, into the columns
 //     directly in front of the tile: buf[plane][LS - lookback .. LS) | tile columns [LS .. LS + T).  Every dilated tap
@@ -225,6 +230,24 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                "l"(src_gmem), "r"(bytes), "r"(smem_addr(bar))
                : "memory");
 }
+// L2 policy of data streamed once (a call's input and output): evicted first, so that it does not push out the rings, which
+// the stream's next tile reads again
+__device__ __forceinline__ u64 l2_evict_first_policy()
+{
+  u64 pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ float ld_streamed(const float* a, const u64 pol)
+{
+  float v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(a), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void st_streamed(float* a, const float v, const u64 pol)
+{
+  asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(a), "f"(v), "l"(pol) : "memory");
+}
 // shared -> global, tracked by the issuing thread's bulk async-group
 __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, u32 bytes)
 {
@@ -304,6 +327,30 @@ __device__ __forceinline__ void static_for(F&& f)
   }
 }
 
+#ifdef NAMB200_SPEC_PROBE
+// Attribution probe (defined by tools/spec_proto only): lane 0 of every warp adds clock64 deltas to spec_probe[]:
+//   [3u] the history wait of unit u, [3u + 1] its B0, [3u + 2] its B1 (u: the layer; NL + a: the convolutional head of
+//   array a), [3 (NL + 2)] whole tiles, [3 (NL + 2) + 1] the number of warp-tiles
+__device__ unsigned long long spec_probe[3 * (spec::NL + 2) + 2];
+#define SPEC_PROBE_START(t) const long long t = clock64()
+#define SPEC_PROBE_ADD(slot, t)                                                                                       \
+  do                                                                                                                  \
+  {                                                                                                                   \
+    if ((threadIdx.x & 31) == 0)                                                                                      \
+      atomicAdd(&spec_probe[slot], (unsigned long long)(clock64() - (t)));                                            \
+  } while (0)
+#define SPEC_PROBE_COUNT(slot)                                                                                        \
+  do                                                                                                                  \
+  {                                                                                                                   \
+    if ((threadIdx.x & 31) == 0)                                                                                      \
+      atomicAdd(&spec_probe[slot], 1ull);                                                                             \
+  } while (0)
+#else
+#define SPEC_PROBE_START(t)
+#define SPEC_PROBE_ADD(slot, t)
+#define SPEC_PROBE_COUNT(slot)
+#endif
+
 struct TileCtx
 {
   float4* buf; // staging buffer: [plane][W] columns
@@ -370,9 +417,13 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
     constexpr int w_conv = Ld.w_off, w_bias = w_conv + K * C * C, w_mix = w_bias + C, w_p = w_mix + C,
                   w_pb = w_p + C * C;
 
+    SPEC_PROBE_START(tb0);
     fence_async_smem(); // my tile columns (generic stores) -> the bulk store below
     __syncthreads(); // B0: the layer input is complete in the tile
+    SPEC_PROBE_ADD(3 * LI + 1, tb0);
+    SPEC_PROBE_START(tw);
     mbar_wait(c.bar, c.phase); // .. and its history has landed in front of it
+    SPEC_PROBE_ADD(3 * LI, tw);
     c.phase ^= 1u;
     if (c.warp == 0) // newest columns -> ring (reads the tile until B1)
       hist_store<P, L, Ld.ring_mask, W>(c.buf, c.state + Ld.ring_off, c.tabs0, c.tv, c.lane);
@@ -402,9 +453,11 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
 #pragma unroll
     for (int q = 0; q < C / 2; q++) // model.cpp:530 (packed add over channel pairs: half the issue slots)
       unpack2(add2(pack2(head[2 * q], head[2 * q + 1]), pack2(acc[2 * q], acc[2 * q + 1])), head[2 * q], head[2 * q + 1]);
+    SPEC_PROBE_START(tb1);
     if (c.warp == 0 && c.lane < P)
       bulk_wait_all(); // my ring stores are done: the tile may be rewritten, the rings may be re-read
     __syncthreads(); // B1: every tap read of this layer's input is done
+    SPEC_PROBE_ADD(3 * LI + 2, tb1);
     // the next unit's history lands under this layer's 1x1 phase
     if constexpr (!last)
       request_layer_history<AI, NT>(c, IntC<LI + 1>{});
@@ -460,9 +513,13 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
       const float q[4] = {head[4 * pl], head[4 * pl + 1], head[4 * pl + 2], head[4 * pl + 3]};
       store_plane<W>(col0, pl, q);
     }
+    SPEC_PROBE_START(tb0);
     fence_async_smem();
     __syncthreads(); // the accumulator columns are complete in the tile
+    SPEC_PROBE_ADD(3 * (spec::NL + AI) + 1, tb0);
+    SPEC_PROBE_START(tw);
     mbar_wait(c.bar, c.phase);
+    SPEC_PROBE_ADD(3 * (spec::NL + AI), tw);
     c.phase ^= 1u;
     if (c.warp == 0)
       hist_store<P, HL, A.head_ring_mask, W>(c.buf, c.state + A.head_ring_off, c.tabs0, c.tv, c.lane);
@@ -485,9 +542,11 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
             headout[ho] = fmaf(spec::w(A.head_off + (k * C + 4 * pl + i) * HOUT + ho), x[i], headout[ho]);
       }
     }
+    SPEC_PROBE_START(tb1);
     if (c.warp == 0 && c.lane < P)
       bulk_wait_all();
     __syncthreads(); // every read of the accumulator columns is done
+    SPEC_PROBE_ADD(3 * (spec::NL + AI) + 2, tb1);
     if constexpr (NEXT_AI >= 0)
       request_layer_history<NEXT_AI, NT>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
     return;
@@ -527,6 +586,7 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  const u64 io_pol = l2_evict_first_policy();
 
   const int batch = p.batch;
   for (int s = blockIdx.x; s < batch; s += gridDim.x)
@@ -540,11 +600,12 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
     c.state = state;
     for (int t0 = 0; t0 < n; t0 += T)
     {
+      SPEC_PROBE_START(ttile);
       c.tv = min(T, n - t0);
       c.tabs0 = clock + (u32)t0;
       request_layer_history<0, NT>(c, IntC<spec::A[0].layer0>{});
       float x[1];
-      x[0] = (tid < c.tv) ? __ldg(xin + t0 + tid) : 0.0f;
+      x[0] = (tid < c.tv) ? ld_streamed(xin + t0 + tid, io_pol) : 0.0f;
       const float cond = x[0]; // no condition_dsp: condition == input (model.cpp:781)
       float y;
       constexpr int C0 = spec::A[0].C;
@@ -573,8 +634,10 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
       }
       // model.cpp:888-897
       if (tid < c.tv)
-        yout[t0 + tid] = spec::head_scale * y;
+        st_streamed(yout + t0 + tid, spec::head_scale * y, io_pol);
       // (no barrier here: the last layer's B1 already fenced every tap read before anything of the next tile is written)
+      SPEC_PROBE_ADD(3 * (spec::NL + 2), ttile);
+      SPEC_PROBE_COUNT(3 * (spec::NL + 2) + 1);
     }
   }
 }
@@ -601,13 +664,6 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
 #ifndef NAMB200_SHORT_PREFETCH
 #define NAMB200_SHORT_PREFETCH 0
 #endif
-
-__device__ __forceinline__ unsigned long long l2_evict_first_policy()
-{
-  unsigned long long pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
 
 __device__ __forceinline__ float4 ring_load(const float4* a, const unsigned long long pol)
 {
@@ -859,10 +915,10 @@ __device__ __forceinline__ void wavenet_spec_short_body(const JitParams& p)
 
 #ifndef NAMB200_SPEC_NO_KERNEL // (wavenet_lat.cuh includes this file for its helpers only)
 #ifndef NAMB200_SPEC_NT
-#define NAMB200_SPEC_NT 512
+#define NAMB200_SPEC_NT 1024
 #endif
 #ifndef NAMB200_SPEC_MINB
-#define NAMB200_SPEC_MINB 2
+#define NAMB200_SPEC_MINB 1
 #endif
 
 // (the entry points are compiled as two NVRTC programs side by side -- jit_spec.cpp: this one and the 64-frame short-call

@@ -1,9 +1,12 @@
 // spec_proto.cu -- stand-alone timing of the model-specialised kernel (wavenet_spec.cuh) on a generated model header.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -I<dir of spec_model.h> -o spec_proto spec_proto.cu
+//   -DNAMB200_SPEC_NT=512 -DNAMB200_SPEC_MINB=2: the two-CTA geometry;  -DNAMB200_SPEC_PROBE: after the timed launches, one
+//   more launch with the kernel's attribution probe, printed as a table of cycles per layer (wavenet_spec.cuh, spec_probe)
 #include <cuda_runtime.h>
 
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <vector>
 
 #include "spec_model.h"
@@ -68,8 +71,39 @@ int main(int argc, char** argv)
   double cs = 0;
   for (size_t i = 0; i < h.size(); i += 997)
     cs += h[i];
+  unsigned long long hash = 1469598103934665603ull; // FNV-1a of every output bit: variants must agree exactly
+  const unsigned char* hb = reinterpret_cast<const unsigned char*>(h.data());
+  for (size_t i = 0; i < h.size() * 4; i++)
+    hash = (hash ^ hb[i]) * 1099511628211ull;
   printf("{\"test\": \"spec_proto\", \"NT\": %d, \"minb\": %d, \"regs\": %d, \"ctas_per_sm\": %d, \"smem\": %zu, \"batch\": %d, "
-         "\"n\": %d, \"ms\": %.3f, \"msamples_per_s\": %.1f, \"checksum\": %.6g}\n",
-         NT, MINB, fa.numRegs, occ, smem, batch, n, best, (double)batch * n / best / 1e3, cs);
+         "\"n\": %d, \"ms\": %.3f, \"msamples_per_s\": %.1f, \"checksum\": %.6g, \"hash\": \"%016llx\"}\n",
+         NT, MINB, fa.numRegs, occ, smem, batch, n, best, (double)batch * n / best / 1e3, cs, hash);
+#ifdef NAMB200_SPEC_PROBE
+  // per unit (layer, or an array's convolutional head): clock64 cycles of its history wait, its B0 and its B1, per warp and
+  // tile, and their share of all warp cycles spent in tiles
+  constexpr int NS = 3 * (spec::NL + 2) + 2;
+  std::vector<unsigned long long> pr(NS, 0ull);
+  CK(cudaMemcpyToSymbol(namb200_spec::spec_probe, pr.data(), NS * 8));
+  wavenet_spec_kernel<<<grid, NT, smem>>>(p);
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpyFromSymbol(pr.data(), namb200_spec::spec_probe, NS * 8));
+  const double wt = (double)pr[NS - 1], tile = (double)pr[NS - 2];
+  printf("probe NT=%d minb=%d: %.0f warp-tiles, %.0f cycles per tile, %.1f cycles per frame per SM\n", NT, MINB, wt, tile / wt,
+         tile / wt / ((double)NT * occ));
+  printf("%-6s %10s %10s %10s %8s %8s %8s\n", "unit", "wait", "B0", "B1", "wait%", "B0%", "B1%");
+  double sum[3] = {0, 0, 0};
+  for (int u = 0; u < spec::NL + 2; u++)
+  {
+    const double v[3] = {(double)pr[3 * u], (double)pr[3 * u + 1], (double)pr[3 * u + 2]};
+    if (v[0] + v[1] + v[2] == 0.0)
+      continue;
+    for (int k = 0; k < 3; k++)
+      sum[k] += v[k];
+    printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%%\n", u < spec::NL ? std::to_string(u).c_str() : ("head" + std::to_string(u - spec::NL)).c_str(),
+           v[0] / wt, v[1] / wt, v[2] / wt, 100 * v[0] / tile, 100 * v[1] / tile, 100 * v[2] / tile);
+  }
+  printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%%\n", "all", sum[0] / wt, sum[1] / wt, sum[2] / wt, 100 * sum[0] / tile,
+         100 * sum[1] / tile, 100 * sum[2] / tile);
+#endif
   return 0;
 }
