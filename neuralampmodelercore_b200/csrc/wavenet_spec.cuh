@@ -109,11 +109,13 @@ __device__ __forceinline__ u64 dup2(float v)
 }
 // the reference's rational fast_tanh (activations.h:91-98) on a packed pair.  The denominator's |x + c x |x|| is
 // evaluated as |x| + c x^2 (the same number: c > 0, so the factor 1 + c |x| is positive; one rounding differs, < 1e-7
-// relative): one packed multiply and one 64-bit AND fewer per pair than the literal form in wavenet_fused.cuh.
+// relative): one packed multiply fewer per pair than the literal form in wavenet_fused.cuh.  |x| is taken per scalar, so
+// that ptxas folds it into the operands of the instructions that use it instead of emitting a 64-bit AND.
 __device__ __forceinline__ u64 fast_tanh2(u64 x)
 {
-  constexpr u64 kAbs = 0x7FFFFFFF7FFFFFFFull;
-  const u64 ax = x & kAbs;
+  float xl, xh;
+  unpack2(x, xl, xh);
+  const u64 ax = pack2(fabsf(xl), fabsf(xh));
   const u64 x2 = mul2(x, x);
   const u64 c0 = dup2(2.45550750702956f);
   const u64 t1 = fma2(dup2(0.821226666969744f), ax, dup2(0.893229853513558f));
@@ -311,6 +313,15 @@ __device__ __forceinline__ void hist_store(const float4* buf, float* ring_f, con
   }
 }
 
+// The tile columns [tv - L, tv) are all that a unit's bulk store reads: only their threads need to order their generic
+// stores before it (the other threads' columns are read by generic loads alone, which B0 orders)
+template <int L>
+__device__ __forceinline__ void fence_stored_columns(const int tv)
+{
+  if (L > 0 && (int)threadIdx.x >= tv - L)
+    fence_async_smem();
+}
+
 // compile-time loop over the layers of an array
 template <int V>
 struct IntC
@@ -329,9 +340,13 @@ __device__ __forceinline__ void static_for(F&& f)
 
 #ifdef NAMB200_SPEC_PROBE
 // Attribution probe (defined by tools/spec_proto only): lane 0 of every warp adds clock64 deltas to spec_probe[]:
-//   [3u] the history wait of unit u, [3u + 1] its B0, [3u + 2] its B1 (u: the layer; NL + a: the convolutional head of
-//   array a), [3 (NL + 2)] whole tiles, [3 (NL + 2) + 1] the number of warp-tiles
-__device__ unsigned long long spec_probe[3 * (spec::NL + 2) + 2];
+//   [5u] the history wait of unit u, [5u + 1] its B0, [5u + 2] its B1 (u: the layer; NL + a: the convolutional head of
+//   array a), [5u + 3] / [5u + 4] how many cycles later warp 0 arrives at B0 / B1 than the CTA's median warp (summed
+//   over CTA-tiles), [5 (NL + 2)] whole tiles, [5 (NL + 2) + 1] the number of warp-tiles.
+// Each warp stores its arrival clocks in shared memory (two buffers, by tile parity); at the end of a tile every warp takes
+// one or two (unit, barrier) pairs of the tile and adds warp 0's lateness, so that no warp carries the bookkeeping.
+__device__ unsigned long long spec_probe[5 * (spec::NL + 2) + 2];
+__shared__ long long spec_probe_arrival[2][2 * (spec::NL + 2)][32]; // [tile parity][2 unit + barrier][warp]
 #define SPEC_PROBE_START(t) const long long t = clock64()
 #define SPEC_PROBE_ADD(slot, t)                                                                                       \
   do                                                                                                                  \
@@ -345,10 +360,46 @@ __device__ unsigned long long spec_probe[3 * (spec::NL + 2) + 2];
     if ((threadIdx.x & 31) == 0)                                                                                      \
       atomicAdd(&spec_probe[slot], 1ull);                                                                             \
   } while (0)
+// this warp's arrival at barrier k (0: B0, 1: B1) of unit u
+#define SPEC_PROBE_ARRIVE(u, k)                                                                                       \
+  do                                                                                                                  \
+  {                                                                                                                   \
+    if ((threadIdx.x & 31) == 0)                                                                                      \
+      spec_probe_arrival[c.probe_parity][2 * (u) + (k)][threadIdx.x >> 5] = clock64();                                \
+  } while (0)
+// at the end of a tile (every warp has waited at the last unit's B1, so every arrival of the tile is visible)
+__device__ __forceinline__ void spec_probe_lateness(const int parity)
+{
+  const int nw = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int pair = warp; pair < 2 * (spec::NL + 2); pair += nw)
+  {
+    const long long mine = lane < nw ? spec_probe_arrival[parity][pair][lane] : 0;
+    if (__shfl_sync(0xffffffffu, mine, 0) == 0) // (a unit this model does not have)
+      continue;
+    int before = 0;
+    for (int j = 0; j < nw; j++)
+    {
+      const long long v = __shfl_sync(0xffffffffu, mine, j);
+      before += v < mine || (v == mine && j < lane);
+    }
+    const unsigned med_lane = __ffs(__ballot_sync(0xffffffffu, lane < nw && before == nw / 2)) - 1;
+    const long long med = __shfl_sync(0xffffffffu, mine, med_lane), w0 = __shfl_sync(0xffffffffu, mine, 0);
+    if (lane == 0)
+      atomicAdd(&spec_probe[5 * (pair >> 1) + 3 + (pair & 1)], (unsigned long long)(w0 - med));
+  }
+}
+#define SPEC_PROBE_TILE_END()                                                                                         \
+  do                                                                                                                  \
+  {                                                                                                                   \
+    spec_probe_lateness(c.probe_parity);                                                                              \
+    c.probe_parity ^= 1;                                                                                              \
+  } while (0)
 #else
 #define SPEC_PROBE_START(t)
 #define SPEC_PROBE_ADD(slot, t)
 #define SPEC_PROBE_COUNT(slot)
+#define SPEC_PROBE_ARRIVE(u, k)
+#define SPEC_PROBE_TILE_END()
 #endif
 
 struct TileCtx
@@ -360,6 +411,9 @@ struct TileCtx
   u32 tabs0; // absolute frame number of the tile's first frame
   int tv; // valid frames in this tile
   int warp, lane;
+#ifdef NAMB200_SPEC_PROBE
+  int probe_parity; // which of the two arrival buffers this tile fills
+#endif
 };
 
 // history of the unit that follows (AI, LI) in program order is requested right after the current unit's last read
@@ -418,12 +472,13 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
                   w_pb = w_p + C * C;
 
     SPEC_PROBE_START(tb0);
-    fence_async_smem(); // my tile columns (generic stores) -> the bulk store below
+    SPEC_PROBE_ARRIVE(LI, 0);
+    fence_stored_columns<L>(c.tv); // my tile columns (generic stores) -> the bulk store below
     __syncthreads(); // B0: the layer input is complete in the tile
-    SPEC_PROBE_ADD(3 * LI + 1, tb0);
+    SPEC_PROBE_ADD(5 * LI + 1, tb0);
     SPEC_PROBE_START(tw);
     mbar_wait(c.bar, c.phase); // .. and its history has landed in front of it
-    SPEC_PROBE_ADD(3 * LI, tw);
+    SPEC_PROBE_ADD(5 * LI, tw);
     c.phase ^= 1u;
     if (c.warp == 0) // newest columns -> ring (reads the tile until B1)
       hist_store<P, L, Ld.ring_mask, W>(c.buf, c.state + Ld.ring_off, c.tabs0, c.tv, c.lane);
@@ -456,8 +511,9 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
     SPEC_PROBE_START(tb1);
     if (c.warp == 0 && c.lane < P)
       bulk_wait_all(); // my ring stores are done: the tile may be rewritten, the rings may be re-read
+    SPEC_PROBE_ARRIVE(LI, 1);
     __syncthreads(); // B1: every tap read of this layer's input is done
-    SPEC_PROBE_ADD(3 * LI + 2, tb1);
+    SPEC_PROBE_ADD(5 * LI + 2, tb1);
     // the next unit's history lands under this layer's 1x1 phase
     if constexpr (!last)
       request_layer_history<AI, NT>(c, IntC<LI + 1>{});
@@ -514,12 +570,13 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
       store_plane<W>(col0, pl, q);
     }
     SPEC_PROBE_START(tb0);
-    fence_async_smem();
+    SPEC_PROBE_ARRIVE(spec::NL + AI, 0);
+    fence_stored_columns<HL>(c.tv);
     __syncthreads(); // the accumulator columns are complete in the tile
-    SPEC_PROBE_ADD(3 * (spec::NL + AI) + 1, tb0);
+    SPEC_PROBE_ADD(5 * (spec::NL + AI) + 1, tb0);
     SPEC_PROBE_START(tw);
     mbar_wait(c.bar, c.phase);
-    SPEC_PROBE_ADD(3 * (spec::NL + AI), tw);
+    SPEC_PROBE_ADD(5 * (spec::NL + AI), tw);
     c.phase ^= 1u;
     if (c.warp == 0)
       hist_store<P, HL, A.head_ring_mask, W>(c.buf, c.state + A.head_ring_off, c.tabs0, c.tv, c.lane);
@@ -545,8 +602,9 @@ __device__ __forceinline__ void array_forward(TileCtx& c, const float (&hin)[spe
     SPEC_PROBE_START(tb1);
     if (c.warp == 0 && c.lane < P)
       bulk_wait_all();
+    SPEC_PROBE_ARRIVE(spec::NL + AI, 1);
     __syncthreads(); // every read of the accumulator columns is done
-    SPEC_PROBE_ADD(3 * (spec::NL + AI) + 2, tb1);
+    SPEC_PROBE_ADD(5 * (spec::NL + AI) + 2, tb1);
     if constexpr (NEXT_AI >= 0)
       request_layer_history<NEXT_AI, NT>(c, IntC<spec::A[NEXT_AI < 0 ? 0 : NEXT_AI].layer0>{});
     return;
@@ -580,6 +638,11 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
   c.phase = 0u;
   c.warp = tid >> 5;
   c.lane = tid & 31;
+#ifdef NAMB200_SPEC_PROBE
+  c.probe_parity = 0;
+  for (int i = tid; i < 2 * 2 * (spec::NL + 2) * 32; i += NT)
+    (&spec_probe_arrival[0][0][0])[i] = 0;
+#endif
   if (tid == 0)
   {
     mbar_init(&bar, 1);
@@ -636,8 +699,9 @@ __device__ __forceinline__ void wavenet_spec_body(const JitParams& p)
       if (tid < c.tv)
         st_streamed(yout + t0 + tid, spec::head_scale * y, io_pol);
       // (no barrier here: the last layer's B1 already fenced every tap read before anything of the next tile is written)
-      SPEC_PROBE_ADD(3 * (spec::NL + 2), ttile);
-      SPEC_PROBE_COUNT(3 * (spec::NL + 2) + 1);
+      SPEC_PROBE_ADD(5 * (spec::NL + 2), ttile);
+      SPEC_PROBE_COUNT(5 * (spec::NL + 2) + 1);
+      SPEC_PROBE_TILE_END();
     }
   }
 }

@@ -80,30 +80,35 @@ int main(int argc, char** argv)
          NT, MINB, fa.numRegs, occ, smem, batch, n, best, (double)batch * n / best / 1e3, cs, hash);
 #ifdef NAMB200_SPEC_PROBE
   // per unit (layer, or an array's convolutional head): clock64 cycles of its history wait, its B0 and its B1, per warp and
-  // tile, and their share of all warp cycles spent in tiles
-  constexpr int NS = 3 * (spec::NL + 2) + 2;
+  // tile, and their share of all warp cycles spent in tiles; then how many cycles later than the CTA's median warp warp 0
+  // arrives at B0 and at B1, per CTA and tile
+  constexpr int NS = 5 * (spec::NL + 2) + 2;
   std::vector<unsigned long long> pr(NS, 0ull);
   CK(cudaMemcpyToSymbol(namb200_spec::spec_probe, pr.data(), NS * 8));
   wavenet_spec_kernel<<<grid, NT, smem>>>(p);
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpyFromSymbol(pr.data(), namb200_spec::spec_probe, NS * 8));
-  const double wt = (double)pr[NS - 1], tile = (double)pr[NS - 2];
+  const double wt = (double)pr[NS - 1], tile = (double)pr[NS - 2], ct = wt / (NT / 32);
   printf("probe NT=%d minb=%d: %.0f warp-tiles, %.0f cycles per tile, %.1f cycles per frame per SM\n", NT, MINB, wt, tile / wt,
          tile / wt / ((double)NT * occ));
-  printf("%-6s %10s %10s %10s %8s %8s %8s\n", "unit", "wait", "B0", "B1", "wait%", "B0%", "B1%");
-  double sum[3] = {0, 0, 0};
+  printf("%-6s %10s %10s %10s %8s %8s %8s %10s %10s\n", "unit", "wait", "B0", "B1", "wait%", "B0%", "B1%", "w0late B0",
+         "w0late B1");
+  double sum[5] = {0, 0, 0, 0, 0};
   for (int u = 0; u < spec::NL + 2; u++)
   {
-    const double v[3] = {(double)pr[3 * u], (double)pr[3 * u + 1], (double)pr[3 * u + 2]};
+    double v[5];
+    for (int k = 0; k < 5; k++)
+      v[k] = (double)(long long)pr[5 * u + k];
     if (v[0] + v[1] + v[2] == 0.0)
       continue;
-    for (int k = 0; k < 3; k++)
+    for (int k = 0; k < 5; k++)
       sum[k] += v[k];
-    printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%%\n", u < spec::NL ? std::to_string(u).c_str() : ("head" + std::to_string(u - spec::NL)).c_str(),
-           v[0] / wt, v[1] / wt, v[2] / wt, 100 * v[0] / tile, 100 * v[1] / tile, 100 * v[2] / tile);
+    printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%% %10.0f %10.0f\n",
+           u < spec::NL ? std::to_string(u).c_str() : ("head" + std::to_string(u - spec::NL)).c_str(), v[0] / wt, v[1] / wt,
+           v[2] / wt, 100 * v[0] / tile, 100 * v[1] / tile, 100 * v[2] / tile, v[3] / ct, v[4] / ct);
   }
-  printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%%\n", "all", sum[0] / wt, sum[1] / wt, sum[2] / wt, 100 * sum[0] / tile,
-         100 * sum[1] / tile, 100 * sum[2] / tile);
+  printf("%-6s %10.0f %10.0f %10.0f %7.2f%% %7.2f%% %7.2f%% %10.0f %10.0f\n", "all", sum[0] / wt, sum[1] / wt, sum[2] / wt,
+         100 * sum[0] / tile, 100 * sum[1] / tile, 100 * sum[2] / tile, sum[3] / ct, sum[4] / ct);
 #endif
   return 0;
 }
