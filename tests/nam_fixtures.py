@@ -99,9 +99,9 @@ def make_wavenet_nam(layers: list[dict], weights, head_scale: float = 1.0, versi
 
 
 def random_wavenet(channels=(16, 8), kernel_size=3, dilations=None, activation="Tanh", seed=0, scale=0.3,
-                   head_bias_last=True, kernel_sizes=None, head_kernel=None, head_dilation=None) -> dict:
+                   head_bias_last=True, kernel_sizes=None, head_kernel=None, head_dilation=None, head_scale=0.02) -> dict:
     """Random-weight plain WaveNet in the a1 family (tools/create_wavenet.py-style), weights U(-scale, scale)
-    like tools/test/test_a2_fast.cpp:109-117."""
+    like tools/test/test_a2_fast.cpp:109-117.  `head_scale` (the last weight) scales the output."""
     from oracle import nam_config
 
     dilations = dilations or [[1, 2, 4, 8], [1, 2, 4, 8]]
@@ -127,13 +127,37 @@ def random_wavenet(channels=(16, 8), kernel_size=3, dilations=None, activation="
         else:
             lc["kernel_size"] = kernel_size
         layers.append(lc)
-    nam = make_wavenet_nam(layers, [], head_scale=0.02)
+    nam = make_wavenet_nam(layers, [], head_scale=head_scale)
     n = nam_config.expected_weight_count(nam)
     rng = np.random.default_rng(seed)
     w = rng.uniform(-scale, scale, size=n).astype(np.float32)
-    w[-1] = 0.02  # head_scale is the last weight
+    w[-1] = head_scale  # head_scale is the last weight
     nam["weights"] = [float(v) for v in w]
     return nam
+
+
+# A centred model (below) still sums its output's constant part in float32 before the head bias removes it: a kernel that
+# sums in another order may differ by a few units in the last place of that part, whatever the centred output's size.
+# Tolerances of centred models add 16 of them (2^-19 of the part removed).
+CENTRED_ROUNDING = 2.0 ** -19
+
+
+def centred(nam: dict, x: np.ndarray, block: int = 64) -> tuple[dict, float]:
+    """`nam` (a random_wavenet whose last head has a bias) with that bias moved so that its output on x ([streams, frames])
+    averages zero, and the mean it removed: a large head_scale then scales the part of the output that follows the input,
+    not a constant offset"""
+    from oracle import oracle
+
+    last = nam["config"]["layers"][-1]
+    assert last.get("head_bias", (last.get("head") or {}).get("bias")), "the last head has no bias"
+    proto = oracle.OracleModel.from_dict(nam)
+    proto.reset(48000.0, block)
+    mean = float(np.mean(proto.run_batch(np.ascontiguousarray(x, np.float32), block)))
+    proto.close()
+    nam = dict(nam, weights=list(nam["weights"]))
+    # the weights end with the last head's bias and head_scale; the output is head_scale x (head + bias)
+    nam["weights"][-2] = float(np.float32(nam["weights"][-2] - mean / nam["weights"][-1]))
+    return nam, mean
 
 
 def make_container(submodels, version: str = "0.7.0", sample_rate: float | None = 48000.0) -> dict:

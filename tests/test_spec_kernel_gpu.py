@@ -76,25 +76,34 @@ def test_call_splitting_and_mixed_kernels_on_one_handle():
 
 
 @pytest.mark.parametrize("case", [
-    dict(channels=(16, 8), kernel_size=3, dilations=[[1, 2, 4, 8, 16, 32], [1, 3, 9, 27, 81]], activation="Tanh"),
-    dict(channels=(8, 4), kernel_sizes=[[2, 3, 4, 5], [5, 2, 3]], dilations=[[1, 7, 13, 64], [2, 5, 128]], activation="ReLU"),
-    dict(channels=(12, 6), kernel_size=3, dilations=[[1, 2, 4, 300], [1, 2, 512]], activation="Sigmoid"),  # padded channels
-    dict(channels=(3,), kernel_size=3, dilations=[[1, 2, 8]], activation="Hardtanh"),  # one array, like wavenet.nam's first
-    dict(channels=(16,), kernel_sizes=[[1, 3, 1, 2]], dilations=[[1, 1, 5, 1024]], activation="SiLU"),  # kernel-size-1 layers: no history
-    dict(channels=(4, 16), kernel_size=4, dilations=[[1, 2], [3, 100, 341]], activation="LeakyReLU"),  # look-back 1023
+    dict(channels=(16, 8), kernel_size=3, dilations=[[1, 2, 4, 8, 16, 32], [1, 3, 9, 27, 81]], activation="Tanh", head_scale=1.5),
+    dict(channels=(8, 4), kernel_sizes=[[2, 3, 4, 5], [5, 2, 3]], dilations=[[1, 7, 13, 64], [2, 5, 128]], activation="ReLU",
+         head_scale=5.0),
+    dict(channels=(12, 6), kernel_size=3, dilations=[[1, 2, 4, 300], [1, 2, 512]], activation="Sigmoid",
+         head_scale=40.0),  # padded channels
+    dict(channels=(3,), kernel_size=3, dilations=[[1, 2, 8]], activation="Hardtanh", head_scale=12.5),  # one array, like wavenet.nam's first
+    dict(channels=(16,), kernel_sizes=[[1, 3, 1, 2]], dilations=[[1, 1, 5, 1024]], activation="SiLU",
+         head_scale=2.0),  # kernel-size-1 layers: no history
+    dict(channels=(4, 16), kernel_size=4, dilations=[[1, 2], [3, 100, 341]], activation="LeakyReLU", head_scale=2.5),  # look-back 1023
 ], ids=["a1_like_odd_dilations", "kernels_2_to_5", "padded_12_6", "single_array", "kernel_1_layers", "narrow_then_wide"])
 def test_shape_family(case):
-    nam = fx.random_wavenet(seed=3, **case)
     B, N = 8, 1400
-    x = fx.synthetic_batch(B, N, seed=2)
+    x = 4.0 * fx.synthetic_batch(B, N, seed=2)  # with each case's head_scale: the output's std over time is above 0.1
+    nam, offset = fx.centred(fx.random_wavenet(seed=3, **case), x)
     ref = _oracle_batch(nam, x, False)
+    assert np.min(np.std(ref, axis=1)) >= 0.1 and np.max(np.abs(ref)) <= 4.0
     d = _spec(nam, B, False)
     d.Reset(48000.0, 1024)
     got = np.concatenate([d.process_batch(np.ascontiguousarray(x[:, p:p + 1024])) for p in range(0, N, 1024)], axis=1)
     d.close()
-    scale = max(1.0, float(np.max(np.abs(ref))))
+    tol = TOL * max(1.0, float(np.max(np.abs(ref)))) + fx.CENTRED_ROUNDING * abs(offset)
     err = float(np.max(np.abs(got - ref)))
-    assert err <= TOL * scale, f"max-abs {err:.3e} (|y| up to {scale:.2f})"
+    assert err <= tol, f"max-abs {err:.3e} (tolerance {tol:.2e})"
+
+
+# the head_scale that puts each model's output std over time above 0.1 (the last head's bias cancels the constant part)
+ACTIVATION_SET_HEAD_SCALE = {"Tanh": 14.0, "Hardtanh": 13.0, "Fasttanh": 14.0, "ReLU": 11.0, "LeakyReLU": 12.0, "PReLU": 12.0,
+                             "Sigmoid": 58.0, "SiLU": 19.0, "Hardswish": 20.0, "LeakyHardtanh": 13.0, "Softsign": 15.0}
 
 
 @pytest.mark.parametrize("act", ["Tanh", "Hardtanh", "Fasttanh", "ReLU", "LeakyReLU", "PReLU", "Sigmoid", "SiLU", "Hardswish",
@@ -108,16 +117,18 @@ def test_activation_set(act):
         activation = {"type": "LeakyHardtanh", "min_val": -0.5, "max_val": 0.7, "min_slope": 0.1, "max_slope": 0.2}
     elif act == "LeakyReLU":
         activation = {"type": "LeakyReLU", "negative_slope": 0.2}
-    nam = fx.random_wavenet(channels=(8,), kernel_size=3, dilations=[[1, 2, 4]], activation=activation, seed=9)
     B, N = 4, 700
     x = fx.synthetic_batch(B, N, seed=8) * 4.0  # drive the saturating activations into both branches
+    nam, offset = fx.centred(fx.random_wavenet(channels=(8,), kernel_size=3, dilations=[[1, 2, 4]], activation=activation,
+                                               seed=9, head_scale=ACTIVATION_SET_HEAD_SCALE[act]), x)
     ref = _oracle_batch(nam, x, False)
+    assert np.min(np.std(ref, axis=1)) >= 0.1 and np.max(np.abs(ref)) <= 4.0  # the output follows the input
     d = _spec(nam, B, False)
     d.Reset(48000.0, N)
     got = d.process_batch(x)
     d.close()
-    scale = max(1.0, float(np.max(np.abs(ref))))
-    assert float(np.max(np.abs(got - ref))) <= TOL * scale
+    tol = TOL * max(1.0, float(np.max(np.abs(ref)))) + fx.CENTRED_ROUNDING * abs(offset)
+    assert float(np.max(np.abs(got - ref))) <= tol
 
 
 def test_prewarmed_state_and_second_reset():
@@ -289,10 +300,13 @@ def test_lat_kernel_irregular_short_calls_several_streams_and_mixing(which, monk
 
 
 @pytest.mark.parametrize("case", [
-    dict(channels=(16, 8), kernel_size=3, dilations=[[1, 2, 4, 8, 16, 32, 64], [1, 3, 9, 27, 81, 200]], activation="Tanh"),
-    dict(channels=(8, 4), kernel_sizes=[[2, 3, 4, 5], [5, 1, 3]], dilations=[[1, 7, 13, 64], [2, 5, 128]], activation="ReLU"),
-    dict(channels=(4, 16), kernel_size=3, dilations=[[1, 2], [3, 100, 341]], activation={"type": "PReLU", "negative_slopes": [0.02 * (i + 1) for i in range(16)]}),
-    dict(channels=(12,), kernel_size=3, dilations=[[1, 2, 40]], activation="Sigmoid"),
+    dict(channels=(16, 8), kernel_size=3, dilations=[[1, 2, 4, 8, 16, 32, 64], [1, 3, 9, 27, 81, 200]], activation="Tanh",
+         head_scale=1.5),
+    dict(channels=(8, 4), kernel_sizes=[[2, 3, 4, 5], [5, 1, 3]], dilations=[[1, 7, 13, 64], [2, 5, 128]], activation="ReLU",
+         head_scale=8.0),
+    dict(channels=(4, 16), kernel_size=3, dilations=[[1, 2], [3, 100, 341]], activation={"type": "PReLU", "negative_slopes": [0.02 * (i + 1) for i in range(16)]},
+         head_scale=1.5),
+    dict(channels=(12,), kernel_size=3, dilations=[[1, 2, 40]], activation="Sigmoid", head_scale=21.0),
 ], ids=["a1_like", "kernels_1_to_5", "prelu_slices", "single_padded_array"])
 @pytest.mark.parametrize("which", ["jit", "precompiled"])
 def test_lat_kernel_shape_family(case, which, monkeypatch):
@@ -302,17 +316,18 @@ def test_lat_kernel_shape_family(case, which, monkeypatch):
     if isinstance(act, dict) and act["type"] == "PReLU":
         # per-array slope counts differ: use a shared slope list sized for the widest array only where it applies
         act = {"type": "PReLU", "negative_slopes": [0.05]}
-    nam = fx.random_wavenet(seed=6, activation=act, **case)
-    x = fx.synthetic_batch(3, 64 * 12, seed=2)
+    x = 4.0 * fx.synthetic_batch(3, 64 * 12, seed=2)  # with each case's head_scale: the output's std over time is above 0.1
+    nam, offset = fx.centred(fx.random_wavenet(seed=6, activation=act, **case), x)
     ref = _oracle_batch(nam, x, False)
+    assert np.min(np.std(ref, axis=1)) >= 0.1 and np.max(np.abs(ref)) <= 4.0
     d = nb.get_dsp(nam, batch=3, jit=3)
     d.Reset(48000.0, 64)
     assert d.jit_lat_state == 1, d.jit_note()
     got = np.concatenate([d.process_batch(np.ascontiguousarray(x[:, p:p + 64])) for p in range(0, x.shape[1], 64)], axis=1)
     d.close()
-    scale = max(1.0, float(np.max(np.abs(ref))))
+    tol = TOL * max(1.0, float(np.max(np.abs(ref)))) + fx.CENTRED_ROUNDING * abs(offset)
     err = float(np.max(np.abs(got - ref)))
-    assert err <= TOL * scale, f"max-abs {err:.3e}"
+    assert err <= tol, f"max-abs {err:.3e} (tolerance {tol:.2e})"
 
 
 def test_short_call_variant_many_streams():
