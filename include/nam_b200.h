@@ -77,7 +77,10 @@ typedef struct nam_b200_options
                   low-latency kernel on handles with few streams and maxBufferSize <= 128 -- the C++ shim's default).  Only calls that take the
                   persistent one-CTA-per-stream path use it; every other mode runs the precompiled kernels on the
                   same state */
-  int32_t reserved[5];
+  int32_t bank_capacity; /* models a bank can hold (nam_b200_create_bank_* only; every other create ignores it): 0 = the
+                            number of documents it is created with; below that, or negative, is refused.  See the model
+                            bank section */
+  int32_t reserved[4];
 } nam_b200_options;
 
 typedef struct nam_b200_info
@@ -199,8 +202,12 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
  *   - ConvNet banks: as an ordinary ConvNet handle (there is no compiled ConvNet kernel).
  *   kernel_geometry 4 (the general kernel) is refused for fused-family and LSTM banks; on a general-WaveNet bank it selects
  *   the precompiled general kernel (as on an ordinary handle), any other non-zero geometry is taken as 4, and a ConvNet bank
- *   ignores it as an ordinary ConvNet handle does.  A bank of one document is exactly nam_b200_create_from_json /
- *   _from_file, JIT included.
+ *   ignores it as an ordinary ConvNet handle does.  A bank of one document and bank_capacity 0 or 1 is exactly
+ *   nam_b200_create_from_json / _from_file, JIT included; with bank_capacity >= 2 it is a bank of K = 1 (precompiled
+ *   kernels, table calls), so that models can be added to it.
+ * Capacity: options.bank_capacity (0 = K) reserves room for that many models at creation; a value below K, or negative, is
+ *   refused with NAM_B200_ERR_INVALID_ARGUMENT.  nam_b200_bank_add_models and _replace_model below never reallocate or
+ *   move what live streams use.
  * All streams start bound to model 0.  Every call of this header works on a bank, each stream exactly (bit for bit) as the
  * same stream of an ordinary jit = 2 handle of its model:
  *   - process calls (nam_b200_process_f32 and _device, process_streams*, the ragged calls, the planar DSP::process on stream
@@ -218,9 +225,11 @@ int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t cap
  *     and an ordinary handle of its model in either direction;
  *   - nam_b200_set_fast_tanh: as on an ordinary handle (an LSTM bank rebuilds its model rows in the new regime before the
  *     next fresh-state copy).
- * Device memory: the K blobs (a1_standard: ~14k floats each; lstm.nam: 64 floats each; a general WaveNet's blob carries
- * its two output scales behind its weights, wavenet_a2_max: ~1.9k floats) and, for fused-family WaveNets, K output scales,
- * plus K "model rows" of state_stride floats each (a1_standard: 196 KB each; lstm.nam: 8 floats) that
+ * Device memory, allocated at creation for C = bank_capacity models: C x (blob + 64-byte record header + model row) plus,
+ * for fused-family WaveNets, C output scales, and a slot table of max(max_batch, C) 16-byte entries (LSTM: max_batch + C).
+ * The C blobs (a1_standard: ~14k floats each; lstm.nam: 64 floats each; a general WaveNet's blob carries
+ * its two output scales behind its weights, wavenet_a2_max: ~1.9k floats), and C "model rows" of state_stride floats
+ * each (a1_standard: 196 KB each, so a capacity of 512 reserves ~130 MB; lstm.nam: 8 floats) that
  * hold every model's freshly reset state (an LSTM's: h0 / c0 plus the prewarm): reset prewarms them together -- an LSTM
  * bank in the same launches as its streams -- and reset_streams and assign_streams copy them (one launch whatever the mix).
  * Cost of mixing: an LSTM kernel's CTA holds several streams (lane groups: 128 / G of them; thread per stream: 64); the
@@ -232,12 +241,31 @@ int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const
 int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out);
 /* K of a bank; 1 for every other handle (so model index 0 is valid on every handle). */
 int nam_b200_bank_size(const nam_b200_model* m);
+/* bank_capacity of a bank (K when it was created with 0); 1 for every other handle. */
+int nam_b200_bank_capacity(const nam_b200_model* m);
+/* Growing a bank: the n documents take model indices K .. K + n - 1 (*first_index = K).  Each is parsed and checked against
+ * model 0 exactly as nam_b200_create_bank_from_json does (same codes and wording; "model k" names the index the document
+ * would receive); more than bank_capacity - K documents, or n < 1, is refused with NAM_B200_ERR_INVALID_ARGUMENT.  All or
+ * nothing: every document is checked before any device work, and a refusal leaves the handle unchanged.  After a reset the
+ * new model rows are prepared at once, each in the state nam_b200_reset would have left it in (current max_frames,
+ * prewarm_on_reset, fast-tanh regime); only those rows are written -- no stream's state or clock changes and no existing
+ * model row is recomputed.  Before the first reset they wait for it.  A general-WaveNet bank's shape-compiled kernel is
+ * reused as it is (its cache key holds no weight).  Returns when the device work has finished; not real-time safe. */
+int nam_b200_bank_add_models(nam_b200_model* m, const char* const* texts, int n, int32_t* first_index);
+/* Recycling an index: model k takes another document of the bank's shape (checked as above): its blob, output scale,
+ * record fingerprint, nam_b200_bank_model_info (and nam_b200_get_info for k = 0) and, after a reset, its model row.  Refused
+ * with NAM_B200_ERR_STATE while any stream is bound to k (the message names how many and the lowest); move them with
+ * nam_b200_assign_streams first.  The overwrite waits for every earlier call of the handle, on any CUDA stream, so an
+ * asynchronous call still running model k finishes with the old weights.  Afterwards import refuses records of the old
+ * document (unless another index still holds it) and accepts the new one's.  NAM_B200_ERR_UNSUPPORTED on a handle that is
+ * not a bank.  Returns when done. */
+int nam_b200_bank_replace_model(nam_b200_model* m, int k, const char* text);
 /* Bind streams[i] to model models[i] and put it in the state of a freshly reset handle of that model (the reset_streams
  * contract, per model: for an LSTM, reset_streams with fresh = 1 on an ordinary handle of that model); every other stream
  * is untouched.  Checked on the host like the other stream lists (distinct streams in [0, max_batch), model indices in
- * [0, bank_size), after reset); a refusal names the entry.  On an ordinary handle (K = 1), models all 0 is
- * nam_b200_reset_streams with fresh = 0 -- for an LSTM that keeps the running state and prewarms on top, unlike a bank of
- * K >= 2, which restarts the stream from its new model's h0 / c0. */
+ * [0, bank_size), after reset); a refusal names the entry.  On an ordinary handle, models all 0 is
+ * nam_b200_reset_streams with fresh = 0 -- for an LSTM that keeps the running state and prewarms on top, unlike a bank,
+ * which restarts the stream from its new model's h0 / c0. */
 int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, const int32_t* models);
 /* out[i] = the model streams[i] is bound to. */
 int nam_b200_stream_models(const nam_b200_model* m, const int32_t* streams, int n, int32_t* out);

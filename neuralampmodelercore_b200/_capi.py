@@ -23,7 +23,8 @@ class Options(C.Structure):
         ("kernel_geometry", C.c_int32),
         ("tile_mode", C.c_int32),
         ("jit", C.c_int32),
-        ("reserved", C.c_int32 * 5),
+        ("bank_capacity", C.c_int32),
+        ("reserved", C.c_int32 * 4),
     ]
 
 
@@ -113,6 +114,9 @@ EXPORTED_SYMBOLS = [
     "nam_b200_bank_model_info",
     "nam_b200_bank_check_json",
     "nam_b200_bank_jit_prepare_json",
+    "nam_b200_bank_capacity",
+    "nam_b200_bank_add_models",
+    "nam_b200_bank_replace_model",
 ]
 
 
@@ -211,8 +215,12 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_bank_check_json.argtypes = [strv, C.c_int, C.c_char_p, C.c_int64]
     lib.nam_b200_bank_jit_prepare_json.argtypes = [strv, C.c_int, C.c_int, C.c_char_p, C.c_int64]
     lib.nam_b200_bank_jit_prepare_json.restype = C.c_int
+    lib.nam_b200_bank_capacity.argtypes = [vp]
+    lib.nam_b200_bank_add_models.argtypes = [vp, strv, C.c_int, i32p]
+    lib.nam_b200_bank_replace_model.argtypes = [vp, C.c_int, C.c_char_p]
     for name in ("nam_b200_create_bank_from_json", "nam_b200_create_bank_from_files", "nam_b200_bank_size",
-                 "nam_b200_assign_streams", "nam_b200_stream_models", "nam_b200_bank_model_info", "nam_b200_bank_check_json"):
+                 "nam_b200_assign_streams", "nam_b200_stream_models", "nam_b200_bank_model_info", "nam_b200_bank_check_json",
+                 "nam_b200_bank_capacity", "nam_b200_bank_add_models", "nam_b200_bank_replace_model"):
         getattr(lib, name).restype = C.c_int
     for name in ("nam_b200_reset_streams", "nam_b200_copy_streams", "nam_b200_export_streams", "nam_b200_import_streams",
                  "nam_b200_export_streams_device", "nam_b200_import_streams_device", "nam_b200_state_layout_json",

@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <memory>
@@ -562,14 +563,18 @@ struct nam_b200_model
   bool slots_used = false;
   int n_out_of_phase = 0; // streams whose history does not end at t_base (Linear: or sits in the other buffer)
   size_t refs_capacity = 0;
-  // model bank (nam_b200_create_bank_*): bank_size >= 2 WaveNets of one WaveNetPlan, or LSTMs of one shape, each stream
+  // model bank (nam_b200_create_bank_*): bank_size WaveNets of one WaveNetPlan, or LSTMs of one shape, each stream
   // bound to one of them.  d_weights holds their blobs weight_stride floats apart, d_head_scales the WaveNets' output
-  // scales, d_bank_headers their record headers.  State rows max_batch .. max_batch + bank_size - 1 are the models' fresh
+  // scales, d_bank_headers their record headers.  State rows max_batch + k (k < bank_size) are the models' fresh
   // rows: reset prewarms them together (a WaveNet bank then copies them out; an LSTM's streams keep their running state);
   // reset_streams / assign_streams copy them.  Their histories end at fresh_clock.  An LSTM bank's rows were prewarmed in
   // the fast-tanh regime rows_fast_tanh; a switch rebuilds them before the next copy.
-  // Ordinary handles: bank_size 1, stream_model all 0, no extra rows.
+  // is_bank is set by create_bank alone (a bank of bank_capacity > 1 is one even while bank_size == 1).  Everything above
+  // is sized for bank_capacity models at creation, so nam_b200_bank_add_models never moves what live streams use.
+  // Ordinary handles: is_bank false, bank_size and bank_capacity 1, stream_model all 0, no extra rows.
+  bool is_bank = false;
   int bank_size = 1;
+  int bank_capacity = 1;
   std::vector<ModelSpec> bank_specs; // model k's document (bank_size entries; bank_specs[0] is `spec`'s twin)
   std::vector<StateRecordHeader> bank_headers;
   std::vector<int32_t> stream_model;
@@ -1172,7 +1177,7 @@ void launch_wavenet(nam_b200_model* m, const JitParams& call, cudaStream_t st)
   {
     void* args[] = {&jp};
     // (a bank's shape-compiled kernel stages each stream's blob in dynamic shared memory)
-    const size_t smem = m->bank_size > 1 ? (size_t)m->weight_stride * sizeof(float) : 0;
+    const size_t smem = m->is_bank ? (size_t)m->weight_stride * sizeof(float) : 0;
     CUDA_CHECK(cudaLaunchKernel((const void*)m->gen_spec_kernel, dim3(std::max(1, std::min(batch, 16 * m->sm_count))), dim3(kGenTile),
                                 args, smem, st));
     m->launches++;
@@ -1197,7 +1202,7 @@ void launch_wavenet(nam_b200_model* m, const JitParams& call, cudaStream_t st)
     gp.n_frames = n_frames;
     gp.t_base = call.t_base;
     // (a bank: each model's blob with its two output scales behind the weights; its calls always carry a table)
-    const bool bank = m->bank_size > 1;
+    const bool bank = m->is_bank;
     gp.n_weight_floats = bank ? (int)m->weight_stride : (int)((m->n_weight_floats + 3) & ~(size_t)3);
     gp.weight_stride = call.weight_stride;
     gp.scale_off = (int)m->gplan.weights.size();
@@ -1445,9 +1450,9 @@ void setup_generic_bank_kernel(nam_b200_model* m)
       why = "loading the shape-compiled general kernel failed: " + err;
   }
   if (!why.empty())
-    return jit_unavailable(m, "model bank of " + std::to_string(m->bank_size) + " models: " + why, b.ok);
+    return jit_unavailable(m, "model bank of up to " + std::to_string(m->bank_capacity) + " models: " + why, b.ok);
   m->spec_state = 1;
-  m->spec_note = "model bank of " + std::to_string(m->bank_size) + " models: the general kernel compiled for the bank's shape, "
+  m->spec_note = "model bank of up to " + std::to_string(m->bank_capacity) + " models: the general kernel compiled for the bank's shape, "
                  + jit_loaded_note(b);
 }
 
@@ -1495,7 +1500,7 @@ void launch_lstm(nam_b200_model* m, const JitParams& call, cudaStream_t st)
   kp.slots = call.slots;
   // a model bank: the BANK instantiations, which read each position's model from the table (whose host copy is
   // m->h_slots[0, batch)); the kernel family is the one an ordinary handle of the same shape gets
-  const bool bank = m->bank_size > 1;
+  const bool bank = m->is_bank;
   kp.weight_stride = call.weight_stride;
   const int H = ls.hidden;
   if (H <= kLstmGroupMaxHidden && ls.num_layers <= kLstmGroupMaxLayers && kp.in_ch == 1 && kp.out_ch == 1)
@@ -1672,7 +1677,7 @@ void launch_convnet(nam_b200_model* m, const JitParams& call, cudaStream_t st)
   kp.n_weight_floats = (int)((m->n_weight_floats + 3) & ~(size_t)3);
   kp.slots = call.slots;
   kp.weight_stride = call.weight_stride; // (a bank: its calls always carry a table)
-  const bool bank = m->bank_size > 1;
+  const bool bank = m->is_bank;
   const size_t wbytes = (size_t)kp.n_weight_floats * sizeof(float);
   const int grid = std::min(call.batch, 16 * m->sm_count);
   if (wbytes <= 200 * 1024)
@@ -1727,7 +1732,7 @@ void recount_phase(nam_b200_model* m)
 // all its streams).
 bool prefix_needs_table(const nam_b200_model* m, int batch)
 {
-  if (m->bank_size > 1)
+  if (m->is_bank)
     return true;
   if (m->n_out_of_phase == 0)
     return false;
@@ -1850,13 +1855,13 @@ void ensure_pinned(nam_b200_model* m, size_t floats)
 // state rows of the handle: one per stream, plus a bank's model rows
 int state_rows(const nam_b200_model* m)
 {
-  return m->opts.max_batch + (m->bank_size > 1 ? m->bank_size : 0);
+  return m->opts.max_batch + (m->is_bank ? m->bank_capacity : 0);
 }
 
 // model k's document (a bank's; model 0 of an ordinary handle is its own)
 const ModelSpec& model_spec(const nam_b200_model* m, int k)
 {
-  return m->bank_size > 1 ? m->bank_specs[(size_t)k] : m->spec;
+  return m->is_bank ? m->bank_specs[(size_t)k] : m->spec;
 }
 
 // an LSTM's trained initial state (lstm.cpp:24-28) as one state row: per layer h0[H] | c0[H]
@@ -1891,7 +1896,7 @@ void init_state(nam_b200_model* m)
     // h0 / c0 are trained parameters (lstm.cpp:24-28): every stream starts from its model's, as every reference DSP object
     // does (prewarm_on_reset = 0 runs no prewarm to broadcast them); a bank's model row k from model k's
     std::vector<int32_t> models(m->stream_model);
-    for (int k = 0; k < (m->bank_size > 1 ? m->bank_size : 0); k++)
+    for (int k = 0; k < (m->is_bank ? m->bank_size : 0); k++)
       models.push_back(k);
     write_lstm_initial_rows(m, m->d_state, 0, models);
   }
@@ -1951,7 +1956,7 @@ void prewarm(nam_b200_model* m)
   // (a standalone nam_b200_prewarm, or a Reset of an LSTM, which keeps its running state) all of them are prewarmed.
   // (a bank's streams run different models: nam_b200_reset prewarms it through prewarm_bank or prewarm_lstm_bank, a
   // standalone prewarm runs every stream with its own model)
-  const bool identical = m->streams_identical && m->bank_size == 1;
+  const bool identical = m->streams_identical && !m->is_bank;
   prewarm_blocks(m, identical ? 1 : m->opts.max_batch, m->opts.max_batch, [&](const JitParams& c) {
     run_device(m, c.in, c.out, c.batch, c.n_frames, c.in_stride, c.out_stride, m->stream);
   });
@@ -2129,7 +2134,7 @@ void lstm_reset_rows(nam_b200_model* m, const int32_t* streams, int n, bool fres
   if (m->opts.prewarm_on_reset)
     prewarm_blocks(m, n, n, [&](JitParams call) {
       call.state = rows;
-      if (m->bank_size == 1)
+      if (!m->is_bank)
         return launch(m, call, m->stream);
       for (int i = 0; i < n; i++)
         m->h_slots[(size_t)i] = StreamRef{i, 0u, m->stream_model[(size_t)streams[i]], call.n_frames};
@@ -2147,6 +2152,10 @@ void bank_fan_out(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t
 {
   if (m->spec.arch == Arch::LSTM && m->rows_fast_tanh != m->fast_tanh_runtime)
     prewarm_lstm_bank(m, false);
+  // (an asynchronous call on another CUDA stream may still be running these streams under their previous binding: their
+  // rows are rewritten after it)
+  if (m->slots_used)
+    CUDA_CHECK(cudaStreamWaitEvent(st, m->slots_free, 0));
   std::vector<StreamRef> refs((size_t)2 * n);
   for (int i = 0; i < n; i++)
   {
@@ -2229,6 +2238,41 @@ void prewarm_lstm_bank(nam_b200_model* m, bool streams)
     });
   m->rows_fast_tanh = m->fast_tanh_runtime;
   m->streams_identical = false;
+  CUDA_CHECK(cudaStreamSynchronize(m->stream));
+}
+
+// Model rows k0 .. k0 + n - 1 of a bank that has been reset (nam_b200_bank_add_models, _replace_model) take the state
+// nam_b200_reset would have left them in, under the current max_frames, prewarm_on_reset and fast-tanh regime; no other row,
+// no clock and not t_base moves.  A WaveNet / ConvNet row starts from zeros at fresh_clock minus the prewarm's frames, so
+// that it ends at fresh_clock, the clock bank_fan_out gives a stream copied from it (zero rings read the same at any
+// clock, so the row equals one prewarmed at reset).  An LSTM row starts from its model's h0 / c0.  The row of an LSTM bank
+// whose other rows wait for a rebuild in a new regime (rows_fast_tanh) is rebuilt with them.
+void prepare_bank_rows(nam_b200_model* m, int k0, int n)
+{
+  const int B = m->opts.max_batch;
+  const bool lstm = m->spec.arch == Arch::LSTM;
+  if (lstm)
+  {
+    std::vector<int32_t> models((size_t)n);
+    for (int i = 0; i < n; i++)
+      models[(size_t)i] = k0 + i;
+    write_lstm_initial_rows(m, m->d_state, (size_t)(B + k0), models);
+  }
+  else
+    CUDA_CHECK(cudaMemsetAsync(m->d_state + (size_t)(B + k0) * m->state_stride, 0, (size_t)n * m->state_stride * sizeof(float),
+                               m->stream));
+  if (m->opts.prewarm_on_reset)
+  {
+    const int bs = std::max(m->max_frames, 1), ps = m->spec.prewarm_samples;
+    const uint32_t frames = ps > 0 ? (uint32_t)((ps + bs - 1) / bs) * (uint32_t)bs : 0u;
+    uint32_t clock = lstm ? m->fresh_clock : m->fresh_clock - frames;
+    prewarm_blocks(m, n, n, [&](const JitParams& call) {
+      for (int i = 0; i < n; i++)
+        m->h_slots[(size_t)i] = StreamRef{B + k0 + i, clock, k0 + i, call.n_frames};
+      launch_with_table(m, call, n, m->stream);
+      clock += lstm ? 0u : (uint32_t)call.n_frames;
+    });
+  }
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 
@@ -2665,7 +2709,7 @@ int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i
   if (h.payload_floats != want.payload_floats)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "payload float count " + std::to_string(h.payload_floats)
                                                  + ", the model's record holds " + std::to_string(want.payload_floats));
-  if (m->bank_size > 1)
+  if (m->is_bank)
   {
     for (int k = 0; k < m->bank_size; k++)
       if (h.fingerprint == m->bank_headers[(size_t)k].fingerprint)
@@ -3083,9 +3127,12 @@ std::string general_bank_difference(int k, const ModelSpec& s, const GenericPlan
   return "";
 }
 
-BankCheck check_bank(const std::vector<ModelSpec>& specs)
+// specs[0] is model 0; specs[k] (k >= 1) is named model k + offset in refusals (nam_b200_bank_add_models checks its
+// documents against model 0 under the indices they would receive)
+BankCheck check_bank(const std::vector<ModelSpec>& specs, int offset = 0)
 {
   BankCheck r;
+  auto index = [&](size_t k) { return k == 0 ? 0 : (int)k + offset; };
   auto refuse = [&](int code, const std::string& why) {
     r.code = code;
     r.reason = why;
@@ -3098,7 +3145,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     r.family = KernelFamily::Lstm;
     for (size_t k = 0; k < specs.size(); k++)
     {
-      const std::string mk = "model " + std::to_string(k) + ": ";
+      const std::string mk = "model " + std::to_string(index(k)) + ": ";
       if (specs[k].arch != Arch::LSTM)
         return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture " + specs[k].architecture
                                                   + ": a bank's models share model 0's architecture (LSTM)");
@@ -3108,7 +3155,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
     }
     for (size_t k = 1; k < specs.size(); k++)
     {
-      const std::string d = lstm_bank_difference((int)k, specs[k], specs[0]);
+      const std::string d = lstm_bank_difference(index(k), specs[k], specs[0]);
       if (!d.empty())
         return refuse(NAM_B200_ERR_MODEL, d);
     }
@@ -3118,7 +3165,7 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
   for (size_t k = 0; k < specs.size(); k++)
   {
     const ModelSpec& s = specs[k];
-    const std::string mk = "model " + std::to_string(k) + ": ";
+    const std::string mk = "model " + std::to_string(index(k)) + ": ";
     if (s.arch == Arch::Container)
       return refuse(NAM_B200_ERR_UNSUPPORTED, mk + "architecture: a slimmable document (SlimmableContainer or slimmable "
                                                    "WaveNet); a bank serves plain WaveNets, ConvNets and LSTMs");
@@ -3147,83 +3194,138 @@ BankCheck check_bank(const std::vector<ModelSpec>& specs)
   for (size_t k = 1; k < specs.size(); k++)
   {
     const std::string d = r.family == KernelFamily::Fused
-                            ? bank_difference((int)k, specs[k], r.plans[k], specs[0], r.plans[0])
-                            : general_bank_difference((int)k, specs[k], r.gplans[k], specs[0], r.gplans[0]);
+                            ? bank_difference(index(k), specs[k], r.plans[k], specs[0], r.plans[0])
+                            : general_bank_difference(index(k), specs[k], r.gplans[k], specs[0], r.gplans[0]);
     if (!d.empty())
       return refuse(NAM_B200_ERR_MODEL, d);
   }
   return r;
 }
 
+// Model i of a checked list as the bank stores it: the fused family's packed blob (its output scale goes to d_head_scales),
+// an LSTM's weights, or the general kernel's weights -- a general WaveNet's followed by its net and condition_dsp output
+// scales, which the BANK instantiation reads from the blob (float4 loads of every blob)
+std::vector<float> bank_blob(const BankCheck& bc, const std::vector<ModelSpec>& specs, size_t i)
+{
+  if (bc.family == KernelFamily::Lstm)
+    return lstm_blob(specs[i]);
+  if (bc.family == KernelFamily::Fused)
+    return bc.plans[i].blob;
+  const GenericPlan& gp = bc.gplans[i];
+  std::vector<float> b = gp.weights;
+  if (specs[i].arch == Arch::WaveNet)
+    b.insert(b.end(), {gp.net.head_scale, gp.cond.head_scale});
+  return b;
+}
+
+// specs[i0 ..] (checked in bc) become models k0 .. of the bank: their blobs, output scales and record headers, queued on
+// the handle's stream (the host sources are pageable: each copy stages them before returning).  The caller orders these
+// writes after every reader of the slots they overwrite.
+void upload_bank_models(nam_b200_model* m, const std::vector<ModelSpec>& specs, const BankCheck& bc, size_t i0, int k0)
+{
+  const size_t n = specs.size() - i0, stride = (size_t)m->weight_stride;
+  std::vector<float> blobs(n * stride, 0.0f), scales(n, 0.0f);
+  std::vector<StateRecordHeader> headers(n);
+  for (size_t i = 0; i < n; i++)
+  {
+    const std::vector<float> blob = bank_blob(bc, specs, i0 + i);
+    std::copy(blob.begin(), blob.end(), blobs.begin() + i * stride);
+    if (bc.family == KernelFamily::Fused)
+      scales[i] = bc.plans[i0 + i].head_scale;
+    headers[i] = state_record_header(specs[i0 + i], m->record_floats);
+  }
+  CUDA_CHECK(cudaMemcpyAsync(m->d_weights + (size_t)k0 * stride, blobs.data(), blobs.size() * sizeof(float),
+                             cudaMemcpyHostToDevice, m->stream));
+  if (m->d_head_scales)
+    CUDA_CHECK(cudaMemcpyAsync(m->d_head_scales + k0, scales.data(), n * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+  if (m->state_error.empty())
+  {
+    CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<unsigned char*>(m->d_bank_headers) + (size_t)k0 * kStateHeaderBytes,
+                               headers.data(), n * kStateHeaderBytes, cudaMemcpyHostToDevice, m->stream));
+    m->bank_headers.resize(std::max(m->bank_headers.size(), (size_t)k0 + n));
+    std::copy(headers.begin(), headers.end(), m->bank_headers.begin() + k0);
+  }
+}
+
 // A bank handle: an ordinary handle of model 0 on the precompiled kernels, then the blobs, output scales (WaveNet), record
-// headers and model rows of all K models
-void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const BankCheck& bc)
+// headers and model rows of `capacity` models, the first K of them filled
+void setup_bank(nam_b200_model* m, std::vector<ModelSpec>&& specs, const BankCheck& bc, int capacity)
 {
   const int K = (int)specs.size();
   const bool lstm = bc.family == KernelFamily::Lstm, fused = bc.family == KernelFamily::Fused;
+  m->is_bank = true;
   m->bank_size = K;
-  // model k's blob: the fused family's packed blob (its output scale goes to d_head_scales), an LSTM's weights, or the
-  // general kernel's weights -- a general WaveNet's followed by its net and condition_dsp output scales, which the BANK
-  // instantiation reads from the blob (float4 loads of every blob)
-  auto blob_of = [&](int k) {
-    if (lstm)
-      return lstm_blob(specs[(size_t)k]);
-    if (fused)
-      return bc.plans[(size_t)k].blob;
-    const GenericPlan& gp = bc.gplans[(size_t)k];
-    std::vector<float> b = gp.weights;
-    if (m->spec.arch == Arch::WaveNet)
-      b.insert(b.end(), {gp.net.head_scale, gp.cond.head_scale});
-    return b;
-  };
-  const size_t len0 = blob_of(0).size();
-  m->weight_stride = (long)((len0 + 3) & ~(size_t)3);
-  std::vector<float> blobs((size_t)K * m->weight_stride, 0.0f), scales((size_t)K);
-  for (int k = 0; k < K; k++)
-  {
-    const std::vector<float> blob = blob_of(k);
-    std::copy(blob.begin(), blob.end(), blobs.begin() + (size_t)k * m->weight_stride);
-    if (fused)
-      scales[(size_t)k] = bc.plans[(size_t)k].head_scale;
-  }
+  m->bank_capacity = capacity;
+  m->weight_stride = (long)((bank_blob(bc, specs, 0).size() + 3) & ~(size_t)3);
   CUDA_CHECK(cudaFree(m->d_weights));
   m->d_weights = nullptr;
-  CUDA_CHECK(cudaMalloc(&m->d_weights, blobs.size() * sizeof(float)));
-  CUDA_CHECK(cudaMemcpy(m->d_weights, blobs.data(), blobs.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_CHECK(cudaMalloc(&m->d_weights, (size_t)capacity * m->weight_stride * sizeof(float)));
   if (fused)
-  {
-    CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)K * sizeof(float)));
-    CUDA_CHECK(cudaMemcpy(m->d_head_scales, scales.data(), (size_t)K * sizeof(float), cudaMemcpyHostToDevice));
-  }
+    CUDA_CHECK(cudaMalloc(&m->d_head_scales, (size_t)capacity * sizeof(float)));
+  if (m->state_error.empty())
+    CUDA_CHECK(cudaMalloc(&m->d_bank_headers, (size_t)capacity * kStateHeaderBytes));
   // the model rows behind the streams' rows
   CUDA_CHECK(cudaFree(m->d_state));
   m->d_state = nullptr;
   CUDA_CHECK(cudaMalloc(&m->d_state, (size_t)m->state_stride * state_rows(m) * sizeof(float)));
-  // slot tables of up to max(max_batch, K) positions (prewarm_bank runs the K model rows in one launch); an LSTM bank's
-  // Reset runs the streams and the model rows in one launch
-  const size_t n_slots = lstm ? (size_t)m->opts.max_batch + K : (size_t)std::max(m->opts.max_batch, K);
+  // slot tables of up to max(max_batch, capacity) positions (prewarm_bank runs the model rows in one launch); an LSTM
+  // bank's Reset runs the streams and the model rows in one launch
+  const size_t n_slots = lstm ? (size_t)m->opts.max_batch + capacity : (size_t)std::max(m->opts.max_batch, capacity);
   m->h_slots.assign(n_slots, StreamRef{0, 0u, 0, 0});
   CUDA_CHECK(cudaFree(m->d_slots));
   m->d_slots = nullptr;
   CUDA_CHECK(cudaMalloc(&m->d_slots, n_slots * sizeof(StreamRef)));
-  if (m->state_error.empty())
-  {
-    for (int k = 0; k < K; k++)
-      m->bank_headers.push_back(state_record_header(specs[(size_t)k], m->record_floats));
-    CUDA_CHECK(cudaMalloc(&m->d_bank_headers, (size_t)K * kStateHeaderBytes));
-    CUDA_CHECK(cudaMemcpy(m->d_bank_headers, m->bank_headers.data(), (size_t)K * kStateHeaderBytes, cudaMemcpyHostToDevice));
-  }
+  upload_bank_models(m, specs, bc, 0, 0);
   m->bank_specs = std::move(specs);
   m->spec_state = 0;
-  m->spec_note = "model bank of " + std::to_string(K) + " models: the precompiled kernels, which read each stream's weights as "
-                 "data (a model-specialised kernel compiles one model's weights into its code)";
+  m->spec_note = "model bank of up to " + std::to_string(capacity) + " models: the precompiled kernels, which read each "
+                 "stream's weights as data (a model-specialised kernel compiles one model's weights into its code)";
   if (bc.family == KernelFamily::General)
     setup_generic_bank_kernel(m); // (throws under jit = 1 when the shape-compiled kernel cannot be had)
   init_state(m);
   CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 
-int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opts, nam_b200_model** out)
+// nam_b200_options::bank_capacity of a bank of n_models documents (0 = n_models), or the refusal
+int bank_capacity_option(const nam_b200_options* opts, int n_models, int* capacity)
+{
+  const bool has = opts && (size_t)std::max(opts->struct_size, 0) >= offsetof(nam_b200_options, bank_capacity) + sizeof(int32_t);
+  const int c = has ? opts->bank_capacity : 0;
+  if (c < 0 || (c > 0 && c < n_models))
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: bank_capacity = " + std::to_string(c) + " must be 0 (the number of "
+                                                 "documents) or >= n_models = " + std::to_string(n_models));
+  *capacity = std::max(c, n_models);
+  return NAM_B200_OK;
+}
+
+// Documents -> the specs of a bank's models; "model k" in a refusal is first + i for texts[i]
+int bank_specs_from_texts(const char* const* texts, int n, int first, bool fast_tanh, const std::string& what,
+                          std::vector<ModelSpec>* specs)
+{
+  LoadOptions lo;
+  lo.fast_tanh = fast_tanh;
+  for (int i = 0; i < n; i++)
+  {
+    const std::string mk = what + "model " + std::to_string(first + i) + ": ";
+    if (!texts[i])
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, mk + "null document");
+    try
+    {
+      specs->push_back(model_spec_from_text(texts[i], lo));
+    }
+    catch (const json::ParseError& ex)
+    {
+      return fail(NAM_B200_ERR_FILE, mk + ex.what());
+    }
+    catch (const std::exception& ex)
+    {
+      return fail(NAM_B200_ERR_MODEL, mk + ex.what());
+    }
+  }
+  return NAM_B200_OK;
+}
+
+int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opts, int capacity, nam_b200_model** out)
 {
   const BankCheck bc = check_bank(specs);
   if (bc.code != NAM_B200_OK)
@@ -3257,7 +3359,7 @@ int create_bank(std::vector<ModelSpec>&& specs, const nam_b200_options* user_opt
   if (bc.family == KernelFamily::General)
     m->opts.jit = user_jit;
   const int rc2 = guarded(m.get(), [&]() -> int {
-    setup_bank(m.get(), std::move(specs), bc);
+    setup_bank(m.get(), std::move(specs), bc, capacity);
     return NAM_B200_OK;
   });
   if (rc2 == NAM_B200_OK)
@@ -3561,7 +3663,7 @@ int nam_b200_get_info(const nam_b200_model* m, nam_b200_info* info)
   m = active_model(m);
   if (!m || !info)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null argument");
-  return fill_info(m, m->spec, info);
+  return fill_info(m, model_spec(m, 0), info); // (a bank: model 0's document, which nam_b200_bank_replace_model may change)
 }
 
 int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
@@ -3602,14 +3704,14 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
       init_state(m);
     m->is_reset = true;
     CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-    if (m->bank_size > 1 && m->spec.arch == Arch::LSTM)
+    if (m->is_bank && m->spec.arch == Arch::LSTM)
       prewarm_lstm_bank(m, true); // (also rebuilds the model rows when prewarm_on_reset = 0: h0 / c0)
     else if (m->opts.prewarm_on_reset)
-      (m->bank_size > 1 ? prewarm_bank : prewarm)(m);
+      (m->is_bank ? prewarm_bank : prewarm)(m);
     CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
     // every stream is now in the state of a freshly reset one: keep stream 0's record for nam_b200_reset_streams (an LSTM
     // keeps its running state across a Reset, so its streams are re-derived per call instead; a bank keeps model rows)
-    if (m->spec.arch != Arch::LSTM && m->state_error.empty() && m->bank_size == 1)
+    if (m->spec.arch != Arch::LSTM && m->state_error.empty() && !m->is_bank)
     {
       const int32_t s0 = 0;
       export_records(m, &s0, 1, m->d_fresh, 0, m->stream);
@@ -3651,9 +3753,9 @@ int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int
       rc = check_stream_list(m, streams, n, "streams", true);
     if (rc != NAM_B200_OK || n == 0)
       return rc;
-    if (m->spec.arch == Arch::LSTM && !(m->bank_size > 1 && fresh))
+    if (m->spec.arch == Arch::LSTM && !(m->is_bank && fresh))
       lstm_reset_rows(m, streams, n, fresh != 0);
-    else if (m->bank_size > 1)
+    else if (m->is_bank)
       bank_fan_out(m, streams, n, m->stream); // each stream's own model's fresh row
     else
       import_records(m, streams, n, m->d_fresh, 0, m->stream); // (fresh or not: Reset forgets the past)
@@ -3857,30 +3959,16 @@ int nam_b200_create_bank_from_json(const char* const* texts, int n_models, const
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: n_models = " + std::to_string(n_models) + " must be >= 1");
   if (!texts)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: null document list");
-  if (n_models == 1)
+  int capacity = 0;
+  if (const int rc = bank_capacity_option(opts, n_models, &capacity); rc != NAM_B200_OK)
+    return rc;
+  if (capacity == 1) // (a bank that can only ever hold its one document is the ordinary handle)
     return nam_b200_create_from_json(texts[0], opts, out);
-  LoadOptions lo;
-  lo.fast_tanh = opts ? (opts->fast_tanh != 0) : false;
   std::vector<ModelSpec> specs;
-  for (int k = 0; k < n_models; k++)
-  {
-    const std::string mk = "model bank: model " + std::to_string(k) + ": ";
-    if (!texts[k])
-      return fail(NAM_B200_ERR_INVALID_ARGUMENT, mk + "null document");
-    try
-    {
-      specs.push_back(model_spec_from_text(texts[k], lo));
-    }
-    catch (const json::ParseError& ex)
-    {
-      return fail(NAM_B200_ERR_FILE, mk + ex.what());
-    }
-    catch (const std::exception& ex)
-    {
-      return fail(NAM_B200_ERR_MODEL, mk + ex.what());
-    }
-  }
-  return create_bank(std::move(specs), opts, out);
+  if (const int rc = bank_specs_from_texts(texts, n_models, 0, opts && opts->fast_tanh != 0, "model bank: ", &specs);
+      rc != NAM_B200_OK)
+    return rc;
+  return create_bank(std::move(specs), opts, capacity, out);
 }
 
 int nam_b200_create_bank_from_files(const char* const* paths, int n_models, const nam_b200_options* opts, nam_b200_model** out)
@@ -3892,7 +3980,10 @@ int nam_b200_create_bank_from_files(const char* const* paths, int n_models, cons
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: n_models = " + std::to_string(n_models) + " must be >= 1");
   if (!paths)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "model bank: null path list");
-  if (n_models == 1)
+  int capacity = 0;
+  if (const int rc = bank_capacity_option(opts, n_models, &capacity); rc != NAM_B200_OK)
+    return rc;
+  if (capacity == 1)
     return nam_b200_create_from_file(paths[0], opts, out);
   LoadOptions lo;
   lo.fast_tanh = opts ? (opts->fast_tanh != 0) : false;
@@ -3915,7 +4006,7 @@ int nam_b200_create_bank_from_files(const char* const* paths, int n_models, cons
       return fail(NAM_B200_ERR_MODEL, mk + ex.what());
     }
   }
-  return create_bank(std::move(specs), opts, out);
+  return create_bank(std::move(specs), opts, capacity, out);
 }
 
 int nam_b200_bank_check_json(const char* const* texts, int n_models, char* out, int64_t capacity)
@@ -4008,6 +4099,84 @@ int nam_b200_bank_size(const nam_b200_model* m)
   return m->bank_size;
 }
 
+int nam_b200_bank_capacity(const nam_b200_model* m)
+{
+  m = active_model(m);
+  if (!m)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null model handle");
+  return m->bank_capacity;
+}
+
+int nam_b200_bank_add_models(nam_b200_model* m, const char* const* texts, int n, int32_t* first_index)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    if (!texts || !first_index)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "bank_add_models: null argument");
+    if (n < 1)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "bank_add_models: n = " + std::to_string(n) + " must be >= 1");
+    const int K = m->bank_size;
+    if (n > m->bank_capacity - K)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "bank_add_models: " + std::to_string(n) + " documents do not fit: the bank holds "
+                                                   + std::to_string(K) + " of its bank_capacity = " + std::to_string(m->bank_capacity)
+                                                   + " models");
+    // every document is checked against model 0 before anything changes: a refusal leaves the handle as it was
+    std::vector<ModelSpec> specs{m->bank_specs[0]};
+    int rc = bank_specs_from_texts(texts, n, K, m->opts.fast_tanh != 0, "bank_add_models: ", &specs);
+    if (rc != NAM_B200_OK)
+      return rc;
+    const BankCheck bc = check_bank(specs, K - 1);
+    if (bc.code != NAM_B200_OK)
+      return fail(bc.code, "model bank: " + bc.reason);
+    // (slots K .. K + n - 1 are read by no call yet)
+    upload_bank_models(m, specs, bc, 1, K);
+    m->bank_specs.insert(m->bank_specs.end(), std::make_move_iterator(specs.begin() + 1), std::make_move_iterator(specs.end()));
+    m->bank_size = K + n;
+    if (m->is_reset)
+      prepare_bank_rows(m, K, n); // (before the first reset, nam_b200_reset prepares them with the others)
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    *first_index = K;
+    return NAM_B200_OK;
+  });
+}
+
+int nam_b200_bank_replace_model(nam_b200_model* m, int k, const char* text)
+{
+  m = active_model(m);
+  return guarded(m, [&]() -> int {
+    if (!m->is_bank)
+      return fail(NAM_B200_ERR_UNSUPPORTED, "bank_replace_model: not a model bank (create one with nam_b200_create_bank_*)");
+    if (k < 0 || k >= m->bank_size)
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "bank_replace_model: model index " + std::to_string(k) + " outside [0, bank_size="
+                                                   + std::to_string(m->bank_size) + ")");
+    int bound = 0, lowest = -1;
+    for (size_t s = 0; s < m->stream_model.size(); s++)
+      if (m->stream_model[s] == k && bound++ == 0)
+        lowest = (int)s;
+    if (bound > 0)
+      return fail(NAM_B200_ERR_STATE, "bank_replace_model: " + std::to_string(bound) + " stream(s) are bound to model "
+                                        + std::to_string(k) + " (the lowest: stream " + std::to_string(lowest)
+                                        + "); move them with assign_streams first");
+    std::vector<ModelSpec> specs{m->bank_specs[0]};
+    int rc = bank_specs_from_texts(&text, 1, k, m->opts.fast_tanh != 0, "bank_replace_model: ", &specs);
+    if (rc != NAM_B200_OK)
+      return rc;
+    const BankCheck bc = check_bank(specs, k - 1);
+    if (bc.code != NAM_B200_OK)
+      return fail(bc.code, "model bank: " + bc.reason);
+    // an earlier call of the handle, on any CUDA stream, may still read blob k or row k: every bank call carries a table,
+    // so the last of them is marked by slots_free
+    if (m->slots_used)
+      CUDA_CHECK(cudaStreamWaitEvent(m->stream, m->slots_free, 0));
+    upload_bank_models(m, specs, bc, 1, k);
+    m->bank_specs[(size_t)k] = std::move(specs[1]);
+    if (m->is_reset)
+      prepare_bank_rows(m, k, 1);
+    CUDA_CHECK(cudaStreamSynchronize(m->stream));
+    return NAM_B200_OK;
+  });
+}
+
 int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, const int32_t* models)
 {
   m = active_model(m);
@@ -4023,7 +4192,7 @@ int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, co
                                                    + ": model index outside [0, bank_size=" + std::to_string(m->bank_size) + ")");
     if (rc != NAM_B200_OK || n == 0)
       return rc;
-    if (m->bank_size == 1)
+    if (!m->is_bank)
       return nam_b200_reset_streams(m, streams, n, 0);
     for (int i = 0; i < n; i++)
       m->stream_model[(size_t)streams[i]] = models[i];
@@ -4056,7 +4225,7 @@ int nam_b200_bank_model_info(const nam_b200_model* m, int k, nam_b200_info* info
   if (k < 0 || k >= m->bank_size)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT,
                 "bank_model_info: model index " + std::to_string(k) + " outside [0, bank_size=" + std::to_string(m->bank_size) + ")");
-  return fill_info(m, m->bank_size > 1 ? m->bank_specs[(size_t)k] : m->spec, info);
+  return fill_info(m, model_spec(m, k), info);
 }
 
 int nam_b200_process_f32_device(nam_b200_model* m, const float* in_device, float* out_device, int batch, int n_frames,

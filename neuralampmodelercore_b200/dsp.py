@@ -470,7 +470,7 @@ class DSP:
     def assign_streams(self, streams, models) -> None:
         """Bind streams[i] to model models[i] and give it that model's freshly reset state; other streams are untouched.
         On an ordinary handle, models all 0 is reset_streams (for an LSTM: fresh=False, which keeps the running state); on
-        a bank of K >= 2 it is reset_streams(fresh=True) on an ordinary handle of the new model."""
+        a bank it is reset_streams(fresh=True) on an ordinary handle of the new model."""
         s = self._streams(streams)
         k = np.ascontiguousarray(np.broadcast_to(np.asarray(models, dtype=np.int32), s.shape), dtype=np.int32)
         self._check(self._lib.nam_b200_assign_streams(self._h, self._i32p(s), len(s), self._i32p(k)))
@@ -489,9 +489,33 @@ class DSP:
         self._check(self._lib.nam_b200_bank_model_info(self._h, int(k), C.byref(info)))
         return info
 
+    @property
+    def bank_capacity(self) -> int:
+        """Models this bank can hold (get_dsp_bank's capacity; K when it was created with 0); 1 for an ordinary handle."""
+        n = int(self._lib.nam_b200_bank_capacity(self._h))
+        if n < 0:
+            _raise(n, self._lib)
+        return n
+
+    def add_models(self, configs) -> list:
+        """Add documents (paths, dicts or JSON texts) of the bank's shape as models K, K+1, ...; returns their indices.
+        All or nothing: a document that could not join the bank at creation, or more documents than the capacity leaves
+        room for, raise and leave the bank unchanged.  After a reset the new models' fresh states are prepared at once;
+        no stream's state changes."""
+        arr, keep = _text_array(_documents(configs))
+        first = C.c_int32(0)
+        self._check(self._lib.nam_b200_bank_add_models(self._h, arr, len(keep), C.byref(first)))
+        return list(range(first.value, first.value + len(keep)))
+
+    def replace_model(self, k: int, config) -> None:
+        """Model k takes another document of the bank's shape (path, dict or JSON text).  Refused while a stream is bound
+        to k (move those streams with assign_streams first); waits for every earlier call of the bank to finish with the
+        old weights."""
+        self._check(self._lib.nam_b200_bank_replace_model(self._h, int(k), _documents([config])[0].encode()))
+
 
 def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: Optional[bool], ctas_per_sm: int,
-             kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0):
+             kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0, capacity: int = 0):
     o = _capi.Options()
     lib.nam_b200_default_options(C.byref(o))
     o.device = int(device)
@@ -502,6 +526,7 @@ def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: O
     o.kernel_geometry = int(kernel_geometry)
     o.tile_mode = int(tile_mode)
     o.jit = int(jit)
+    o.bank_capacity = int(capacity)
     return o
 
 
@@ -551,7 +576,7 @@ def _text_array(texts: list):
 
 def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bool] = None,
                  fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
-                 tile_mode: int = 0, jit: int = 0) -> DSP:
+                 tile_mode: int = 0, jit: int = 0, capacity: int = 0) -> DSP:
     """A model bank: one handle of `batch` streams over the K documents in `configs` (paths, dicts or JSON texts), which
     must share one shape (bank_check): WaveNets of the fused kernel family, WaveNets of the general kernel (A2-style,
     condition_dsp, multi-channel), ConvNets, or LSTMs.  Every stream starts bound to model
@@ -562,9 +587,10 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
     bank's shape (bank_jit_prepare; 0 default, 1 required, 2 off, 3 preferred); fused and LSTM banks refuse jit = 1 and
     run the precompiled kernels under 0 / 3; a ConvNet bank takes it as an ordinary ConvNet handle.  kernel_geometry = 4
     is refused for fused-family and LSTM banks; on a general bank it selects the precompiled general kernel, and a
-    ConvNet bank ignores it.  A bank of one document is get_dsp."""
+    ConvNet bank ignores it.  capacity: the models the bank can hold (0 = len(configs)); room for DSP.add_models is
+    reserved at creation.  A bank of one document and capacity 0 or 1 is get_dsp."""
     lib = _capi.load()
-    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit)
+    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit, capacity)
     arr, _keep = _text_array(_documents(configs))
     h = C.c_void_p()
     rc = lib.nam_b200_create_bank_from_json(arr, len(_keep), C.byref(o), C.byref(h))
