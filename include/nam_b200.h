@@ -80,7 +80,20 @@ typedef struct nam_b200_options
   int32_t bank_capacity; /* models a bank can hold (nam_b200_create_bank_* only; every other create ignores it): 0 = the
                             number of documents it is created with; below that, or negative, is refused.  See the model
                             bank section */
-  int32_t reserved[4];
+  union
+  {
+    int32_t reserved[4]; /* the last four words, zero by default; code that zeroes reserved[0..3] keeps compiling and
+                            keeps asking for the defaults */
+    struct
+    {
+      int32_t resample; /* 0 (default) = the host rate given to nam_b200_reset is recorded and ignored, as by the
+                           reference; 1 = convert every stream from that rate to the model's expected rate before the model
+                           and back after it, on the device, in the same call (see the sample-rate conversion section).
+                           Equal rates convert nothing: outputs and launches are then exactly those of 0.  Multi-GPU
+                           handles refuse 1 */
+      int32_t reserved_tail[3];
+    };
+  };
 } nam_b200_options;
 
 typedef struct nam_b200_info
@@ -99,7 +112,9 @@ typedef struct nam_b200_info
   int32_t kernel_variant; /* which CUDA specialisation serves this model (diagnostic) */
   int32_t jit_state; /* model-specialised kernel: 1 = active, 0 = not requested, -1 = requested but unavailable */
   int32_t jit_lat_state; /* the same for the low-latency kernel (few streams, calls of <= 128 frames; built by reset) */
-  int32_t reserved[5];
+  int32_t resample_up, resample_down; /* L and M of the last reset's conversion (model / host = L / M); 1, 1 when none */
+  int32_t resample_latency_frames; /* group delay of the conversion in host frames, rounded (0 when none) */
+  int32_t reserved[2];
 } nam_b200_info;
 
 /* Fill with defaults: device -1, max_batch 1, fast_tanh 0, prewarm_on_reset 1. */
@@ -334,6 +349,44 @@ int nam_b200_process_streams_ragged_f32(nam_b200_model* m, const int32_t* stream
 int nam_b200_process_streams_ragged_f32_device(nam_b200_model* m, const int32_t* streams, int n, const int32_t* n_frames,
                                                const float* in_device, float* out_device, int64_t in_stride,
                                                int64_t out_stride, void* cuda_stream);
+
+/* ---- sample-rate conversion (options.resample = 1) ----------------------------------------------------------------------
+ * When nam_b200_reset gets a sample_rate other than the model's expected rate, every stream is converted from that host
+ * rate to the model's rate before the model and back after it, on the device, in the same call.
+ *   Rates: both must be integers in Hz.  L / M = model_rate / host_rate in lowest terms, L, M <= 1024, and the filter below
+ *     must need at most 128 taps per output sample in each direction (rates within a factor of about 2.5: 44.1 <-> 48 kHz
+ *     takes 58, 96 -> 48 kHz 107, 32 -> 48 kHz 80).  Otherwise, and when the expected rate is unknown (-1), reset fails with
+ *     NAM_B200_ERR_INVALID_ARGUMENT naming both rates.  Equal rates convert nothing.
+ *   Definition: let h be a stream's host-sample count since its last reset.  A call of n host frames makes model samples
+ *     k in [ceil(h L / M), ceil((h + n) L / M)), y[k] = sum_i x[i] g_up[k M - i L], runs the model on them (z), and returns
+ *     host samples j in [h, h + n), out[j] = sum_k z[k] g_dn[j L - k M].  Both sums are causal, so every call returns n
+ *     frames and the result does not depend on how a stream's audio is split into calls (bit for bit: each output sample
+ *     is one fixed-order fmaf chain).  It is scipy.signal.upfirdn(g_up, x, L, M), the model, then upfirdn(g_dn, z, M, L).
+ *   Filter: one Kaiser-windowed sinc at the common rate fs = host_rate * L, designed in double precision and stored as
+ *     float32, g_up = L g, g_dn = M g:  A = 84 dB, beta = 0.1102 (A - 8.7), fmin = min(host_rate, model_rate),
+ *     fc = 0.45 fmin / fs, df = 0.1 fmin / fs (cycles per sample), N = ceil((A - 7.95) / (2.285 * 2 pi df)) + 1,
+ *     g[n] = 2 fc sinc(2 fc (n - (N-1)/2)) I0(beta sqrt(1 - ((n - (N-1)/2) / ((N-1)/2))^2)) / I0(beta), n in [0, N),
+ *     sinc(x) = sin(pi x) / (pi x).  Passband ripple <= 0.1 dB up to 0.4 fmin, stopband >= 80 dB from 0.5 fmin.  Taps per
+ *     output: ceil(N / L) host -> model, ceil(N / M) model -> host.  Latency (both filters): (N - 1) / L host frames.
+ *   max_frames of nam_b200_reset counts host frames; the model's own calls take up to ceil(max_frames L / M) frames, and
+ *     prewarm runs at the model's rate on zeros in blocks of that size (the resampler histories stay zero).
+ *   Every process entry converts: nam_b200_process_f32 and _device, process_streams*, the ragged calls (n_frames[i] are
+ *     host frames; each stream advances its own h, and its model clock by its own count of model frames), the planar
+ *     DSP::process on stream 0 (without the low-latency doorbell) and the host-buffer path (without its chunk pipeline).
+ *     A stream left out of a call, or given 0 frames, keeps its resampler state and h.  A call runs the host -> model
+ *     kernel, the model's launch (the ragged launch of n_max = the longest row's model frames; the contiguous one when
+ *     every row has the same count and no table is needed), the model -> host kernel and one history update.
+ *   State: reset_streams and assign_streams zero a stream's resampler histories and set h = 0; copy_streams carries them.
+ *     A record of a converting handle appends three segments after the model's: resample_in (in_channels x ceil(N / L)
+ *     columns, oldest first), resample_out (out_channels x ceil(N / M) columns), resample_phase (one float, h mod M); its
+ *     header word 3 (bytes 12-15) holds L << 16 | M (0 on a handle that converts nothing).  Import refuses a record whose
+ *     ratio differs from the handle's, naming the field.  nam_b200_stream_state_size therefore follows the last reset.
+ *   Banks share one expected rate, hence one ratio; SlimmableContainer handles pass the option to their sub-models. */
+/* Host-only, no CUDA: the conversion between these rates as a JSON object -- host_rate, model_rate, L, M, n_taps,
+ * taps_per_output_up, taps_per_output_down, latency_frames (host frames, a double), g_up, g_dn (%.9g).  Refuses a pair
+ * exactly as nam_b200_reset does (equal rates included: L = M = 1 is a valid design); NAM_B200_ERR_INVALID_ARGUMENT also
+ * when the buffer is too small. */
+int nam_b200_resampler_json(double host_rate, double model_rate, char* out, int64_t capacity);
 
 /* Host-buffer contract of nam_b200_process_f32: any host memory is accepted; with PAGE-LOCKED buffers (cudaMallocHost,
  * cudaHostRegister, or nam_b200_pin_host_buffer below) the call pipelines host->device copy, kernel and device->host copy

@@ -20,6 +20,7 @@ from .dsp import (  # noqa: F401
     jit_prepare,
     measure_fp32_tflops,
     has_tensor_core_kernel,
+    resampler,
     state_layout,
     submodels,
     using_fast_tanh,
@@ -37,6 +38,7 @@ __all__ = [
     "jit_prepare",
     "submodels",
     "state_layout",
+    "resampler",
     "enable_fast_tanh",
     "disable_fast_tanh",
     "using_fast_tanh",

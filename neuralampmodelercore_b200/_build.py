@@ -17,7 +17,7 @@ LIB_PATH = LIB_DIR / "libnam_b200.so"
 INCLUDE = PKG.parent / "include"
 
 SOURCES = ["nam_b200.cu", "nam_model_spec.cpp", "json_lite.cpp", "wavenet_pack.cpp", "generic_pack.cpp", "nam_dsp_shim.cpp",
-           "jit_spec.cpp", "stream_state.cpp"]
+           "jit_spec.cpp", "stream_state.cpp", "resample.cpp"]
 
 
 def _obj_name(src: Path) -> str:

@@ -12,7 +12,17 @@ f32p = C.POINTER(C.c_float)
 f64p = C.POINTER(C.c_double)
 
 
+class _OptionsWords(C.Structure):
+    _fields_ = [("resample", C.c_int32), ("reserved_tail", C.c_int32 * 3)]
+
+
+class _OptionsTail(C.Union):
+    _anonymous_ = ("_words",)
+    _fields_ = [("reserved", C.c_int32 * 4), ("_words", _OptionsWords)]
+
+
 class Options(C.Structure):
+    _anonymous_ = ("_tail",)
     _fields_ = [
         ("struct_size", C.c_int32),
         ("device", C.c_int32),
@@ -24,7 +34,7 @@ class Options(C.Structure):
         ("tile_mode", C.c_int32),
         ("jit", C.c_int32),
         ("bank_capacity", C.c_int32),
-        ("reserved", C.c_int32 * 4),
+        ("_tail", _OptionsTail),
     ]
 
 
@@ -50,7 +60,10 @@ class Info(C.Structure):
         ("kernel_variant", C.c_int32),
         ("jit_state", C.c_int32),
         ("jit_lat_state", C.c_int32),
-        ("reserved", C.c_int32 * 5),
+        ("resample_up", C.c_int32),
+        ("resample_down", C.c_int32),
+        ("resample_latency_frames", C.c_int32),
+        ("reserved", C.c_int32 * 2),
     ]
 
 
@@ -117,6 +130,7 @@ EXPORTED_SYMBOLS = [
     "nam_b200_bank_capacity",
     "nam_b200_bank_add_models",
     "nam_b200_bank_replace_model",
+    "nam_b200_resampler_json",
 ]
 
 
@@ -218,6 +232,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.nam_b200_bank_capacity.argtypes = [vp]
     lib.nam_b200_bank_add_models.argtypes = [vp, strv, C.c_int, i32p]
     lib.nam_b200_bank_replace_model.argtypes = [vp, C.c_int, C.c_char_p]
+    lib.nam_b200_resampler_json.argtypes = [C.c_double, C.c_double, C.c_char_p, C.c_int64]
+    lib.nam_b200_resampler_json.restype = C.c_int
     for name in ("nam_b200_create_bank_from_json", "nam_b200_create_bank_from_files", "nam_b200_bank_size",
                  "nam_b200_assign_streams", "nam_b200_stream_models", "nam_b200_bank_model_info", "nam_b200_bank_check_json",
                  "nam_b200_bank_capacity", "nam_b200_bank_add_models", "nam_b200_bank_replace_model"):

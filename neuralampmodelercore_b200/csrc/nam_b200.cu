@@ -26,6 +26,8 @@
 #include "wavenet_generic.cuh"
 #include "jit_spec.h"
 #include "stream_state.cuh"
+#include "resample.h"
+#include "resample.cuh"
 
 using namespace namb200;
 
@@ -594,6 +596,27 @@ struct nam_b200_model
   size_t h_pin_floats = 0;
   double flops_per_frame = 0.0;
 
+  // sample-rate conversion (options.resample, resample.cuh), set up by reset when the host rate differs from the model's.
+  // Per stream, one row of rs_stride floats: in_channels x H_up host inputs, then out_channels x H_dn model outputs; row
+  // max_batch stays zero (reset_streams copies it).  phase[s] = h mod M of stream s.  max_frames is then the model's
+  // (ceil(host_max_frames L / M)); the process entries check host frames against host_max_frames.
+  struct Resampler
+  {
+    bool active = false;
+    ResamplerDesign design;
+    int H_up = 0, H_dn = 0, rs_stride = 0;
+    int host_max_frames = 0;
+    std::vector<uint32_t> phase;
+    std::vector<RsPos> h_pos;
+    float* d_taps = nullptr; // phase tables: host -> model ([T_up][L]), then model -> host ([T_dn][M])
+    float* d_hist = nullptr; // (max_batch + 1) rows
+    float* d_x = nullptr; // model-rate input of a call, [position][in_channels][n_max]
+    float* d_z = nullptr; // model-rate output, [position][out_channels][n_max]
+    RsPos* d_pos = nullptr;
+    cudaEvent_t pos_free = nullptr; // recorded after the last launch that reads d_pos
+    bool pos_used = false;
+  } rs;
+
   // host-buffer calls on large batches are pipelined in chunks of streams: H2D(c+1) | kernel(c) | D2H(c-1)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   std::vector<cudaEvent_t> chunk_events;
@@ -641,6 +664,11 @@ struct nam_b200_model
       cudaFree(d_in);
     if (d_out)
       cudaFree(d_out);
+    for (void* p : {(void*)rs.d_taps, (void*)rs.d_hist, (void*)rs.d_x, (void*)rs.d_z, (void*)rs.d_pos})
+      if (p)
+        cudaFree(p);
+    if (rs.pos_free)
+      cudaEventDestroy(rs.pos_free);
     if (h_pin)
       cudaFreeHost(h_pin);
     if (h_flag)
@@ -1851,6 +1879,206 @@ void ensure_pinned(nam_b200_model* m, size_t floats)
   }
 }
 
+// ---- sample-rate conversion (options.resample; resample.h, resample.cuh) ----------------------------------------------
+// host frames a process call may carry: maxBufferSize of the last reset
+int call_max_frames(const nam_b200_model* m)
+{
+  return m->rs.active ? m->rs.host_max_frames : m->max_frames;
+}
+// frames per stream of the host staging buffers: host calls and the model's own calls (prewarm) both pass through them
+int staging_frames(const nam_b200_model* m)
+{
+  return std::max(m->max_frames, call_max_frames(m));
+}
+
+// dynamic shared memory of one conversion launch: the phase table and the input window of `tile` outputs
+size_t rs_smem_bytes(int T, int A, int B, int tile)
+{
+  return 4 * ((size_t)T * B + (size_t)(tile - 1) * A / B + T + 2);
+}
+
+void free_resampler(nam_b200_model* m)
+{
+  auto& r = m->rs;
+  for (float** p : {&r.d_taps, &r.d_hist, &r.d_x, &r.d_z})
+  {
+    if (*p)
+      cudaFree(*p);
+    *p = nullptr;
+  }
+  if (r.d_pos)
+    cudaFree(r.d_pos);
+  r.d_pos = nullptr;
+  r.active = false;
+}
+
+// The conversion nam_b200_reset(host_rate) needs: *d and true, or false when none is (resample = 0, equal rates).
+// Returns the refusal ("" when fine) -- checked before reset changes anything.
+std::string resampler_for(const nam_b200_model* m, double host_rate, ResamplerDesign* d, bool* needed)
+{
+  *needed = m->opts.resample != 0 && host_rate != m->spec.sample_rate;
+  std::string why;
+  if (!*needed)
+    return why;
+  if (design_resampler(host_rate, m->spec.sample_rate, d, &why))
+  {
+    int optin = 0;
+    CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
+    const size_t smem = std::max(rs_smem_bytes(d->taps_up, d->M, d->L, kRsMaxThreads), rs_smem_bytes(d->taps_dn, d->L, d->M, kRsMaxThreads));
+    if (smem > (size_t)optin)
+      why = "resample: host rate " + std::to_string((long long)host_rate) + " Hz, model rate " + std::to_string((long long)m->spec.sample_rate)
+            + " Hz: the phase tables need " + std::to_string(smem) + " bytes of shared memory, more than the device's "
+            + std::to_string(optin);
+  }
+  return why;
+}
+
+// nam_b200_reset's part: every stream's conversion state zero, h = 0; m->max_frames becomes the model's maxBufferSize
+void setup_resampler(nam_b200_model* m, bool needed, const ResamplerDesign& d, int max_frames)
+{
+  free_resampler(m);
+  m->max_frames = max_frames;
+  if (!needed)
+    return;
+  auto& r = m->rs;
+  const int ci = m->spec.in_channels, co = m->spec.out_channels, nb = m->opts.max_batch;
+  r.design = d;
+  r.H_up = d.taps_up;
+  r.H_dn = d.taps_dn;
+  r.rs_stride = (ci * r.H_up + co * r.H_dn + 3) & ~3;
+  r.host_max_frames = max_frames;
+  m->max_frames = (int)(((int64_t)max_frames * d.L + d.M - 1) / d.M);
+  std::vector<float> taps = resampler_phase_table(d.g_up, d.L, d.taps_up);
+  const std::vector<float> dn = resampler_phase_table(d.g_dn, d.M, d.taps_dn);
+  taps.insert(taps.end(), dn.begin(), dn.end());
+  CUDA_CHECK(cudaMalloc(&r.d_taps, taps.size() * sizeof(float)));
+  CUDA_CHECK(cudaMemcpy(r.d_taps, taps.data(), taps.size() * sizeof(float), cudaMemcpyHostToDevice));
+  const size_t hist = (size_t)(nb + 1) * r.rs_stride;
+  CUDA_CHECK(cudaMalloc(&r.d_hist, hist * sizeof(float)));
+  CUDA_CHECK(cudaMemsetAsync(r.d_hist, 0, hist * sizeof(float), m->stream));
+  CUDA_CHECK(cudaMalloc(&r.d_x, (size_t)nb * ci * m->max_frames * sizeof(float)));
+  CUDA_CHECK(cudaMalloc(&r.d_z, (size_t)nb * co * m->max_frames * sizeof(float)));
+  CUDA_CHECK(cudaMalloc(&r.d_pos, (size_t)nb * sizeof(RsPos)));
+  if (!r.pos_free)
+    CUDA_CHECK(cudaEventCreateWithFlags(&r.pos_free, cudaEventDisableTiming));
+  r.pos_used = false;
+  r.phase.assign((size_t)nb, 0u);
+  r.h_pos.assign((size_t)nb, RsPos{0, 0, 0, 0});
+  int optin = 0;
+  CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
+  ensure_max_dynamic_smem((const void*)resample_kernel<true>, m->device, optin);
+  ensure_max_dynamic_smem((const void*)resample_kernel<false>, m->device, optin);
+  r.active = true;
+}
+
+// One direction over the call's positions (m->rs.d_pos): up = host -> model.  n_out_max: the longest output row.
+void launch_resample(nam_b200_model* m, bool up, const float* in, long in_stride, int in_pitch, float* out, long out_stride,
+                     int out_pitch, int n_pos, int n_out_max, cudaStream_t st)
+{
+  if (n_out_max == 0)
+    return;
+  const auto& r = m->rs;
+  const ResamplerDesign& d = r.design;
+  ResampleParams p{};
+  p.T = up ? d.taps_up : d.taps_dn;
+  p.A = up ? d.M : d.L;
+  p.B = up ? d.L : d.M;
+  p.taps = r.d_taps + (up ? 0 : (size_t)d.taps_up * d.L);
+  p.pos = r.d_pos;
+  p.n_pos = n_pos;
+  p.in = in;
+  p.in_stride = in_stride;
+  p.in_pitch = in_pitch;
+  p.out = out;
+  p.out_stride = out_stride;
+  p.out_pitch = out_pitch;
+  p.hist = r.d_hist;
+  p.hist_stride = r.rs_stride;
+  p.hist_off = up ? 0 : m->spec.in_channels * r.H_up;
+  p.H = up ? r.H_up : r.H_dn;
+  const int tile = std::min(kRsMaxThreads, (n_out_max + 31) & ~31);
+  const int tiles = (n_out_max + tile - 1) / tile;
+  const int ch = up ? m->spec.in_channels : m->spec.out_channels;
+  // positions per CTA: about four CTAs per SM in all, so that each stages the phase table once for many rows
+  p.group = (int)std::max<long>(1, (long)n_pos * tiles * ch / (4L * std::max(m->sm_count, 1)));
+  const dim3 grid((unsigned)((n_pos + p.group - 1) / p.group), (unsigned)tiles, (unsigned)ch);
+  const size_t smem = rs_smem_bytes(p.T, p.A, p.B, tile);
+  if (up)
+    resample_kernel<true><<<grid, tile, smem, st>>>(p);
+  else
+    resample_kernel<false><<<grid, tile, smem, st>>>(p);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+}
+
+// run_device for the process entries: on a converting handle, host -> model into rs.d_x, the model's launch over it (per
+// position its own count of model frames), model -> host into d_out, then the histories; otherwise run_device itself.
+// `n_frames` is the call's host frame pitch (the longest row of a ragged call).
+void run_call(nam_b200_model* m, const float* d_in, float* d_out, int batch, int n_frames, long in_stride, long out_stride,
+              cudaStream_t st, const int32_t* streams = nullptr, const int32_t* counts = nullptr)
+{
+  auto& r = m->rs;
+  if (!r.active)
+    return run_device(m, d_in, d_out, batch, n_frames, in_stride, out_stride, st, streams, counts);
+  const int64_t L = r.design.L, M = r.design.M;
+  int m_max = 0;
+  bool equal = true;
+  for (int i = 0; i < batch; i++)
+  {
+    const int s = streams ? streams[i] : i;
+    const int n = counts ? counts[i] : n_frames;
+    const int64_t ph = r.phase[(size_t)s];
+    const int mi = (int)(((ph + n) * L + M - 1) / M - (ph * L + M - 1) / M);
+    r.h_pos[(size_t)i] = RsPos{s, (int)((M - (ph * L) % M) % M), n, mi};
+    m_max = std::max(m_max, mi);
+    equal = equal && mi == r.h_pos[0].m;
+  }
+  if (r.pos_used)
+    CUDA_CHECK(cudaStreamWaitEvent(st, r.pos_free, 0));
+  CUDA_CHECK(cudaMemcpyAsync(r.d_pos, r.h_pos.data(), (size_t)batch * sizeof(RsPos), cudaMemcpyHostToDevice, st));
+  const int ci = m->spec.in_channels, co = m->spec.out_channels;
+  launch_resample(m, true, d_in, in_stride, n_frames, r.d_x, (long)ci * m_max, m_max, batch, m_max, st);
+  if (m_max > 0)
+  {
+    if (!streams && equal)
+      run_device(m, r.d_x, r.d_z, batch, m_max, (long)ci * m_max, (long)co * m_max, st);
+    else
+    {
+      std::vector<int32_t> ids((size_t)batch), cnt((size_t)batch);
+      for (int i = 0; i < batch; i++)
+      {
+        ids[(size_t)i] = r.h_pos[(size_t)i].stream;
+        cnt[(size_t)i] = r.h_pos[(size_t)i].m;
+      }
+      run_device(m, r.d_x, r.d_z, batch, m_max, (long)ci * m_max, (long)co * m_max, st, ids.data(), equal ? nullptr : cnt.data());
+    }
+  }
+  launch_resample(m, false, r.d_z, (long)co * m_max, m_max, d_out, out_stride, n_frames, batch, n_frames, st);
+  ResampleHistoryParams hp{};
+  hp.pos = r.d_pos;
+  hp.in_channels = ci;
+  hp.x = d_in;
+  hp.x_stride = in_stride;
+  hp.x_pitch = n_frames;
+  hp.z = r.d_z;
+  hp.z_stride = (long)co * m_max;
+  hp.z_pitch = m_max;
+  hp.hist = r.d_hist;
+  hp.hist_stride = r.rs_stride;
+  hp.H_up = r.H_up;
+  hp.H_dn = r.H_dn;
+  resample_history_kernel<<<dim3((unsigned)batch, (unsigned)(ci + co)), kRsHistThreads, 0, st>>>(hp);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+  CUDA_CHECK(cudaEventRecord(r.pos_free, st));
+  r.pos_used = true;
+  for (int i = 0; i < batch; i++)
+  {
+    const RsPos& p = r.h_pos[(size_t)i];
+    r.phase[(size_t)p.stream] = (uint32_t)((r.phase[(size_t)p.stream] + (uint32_t)p.n) % (uint32_t)M);
+  }
+}
+
 // Zero the state, set the trained initial state where the architecture has one.
 // state rows of the handle: one per stream, plus a bank's model rows
 int state_rows(const nam_b200_model* m)
@@ -1978,9 +2206,20 @@ void prewarm(nam_b200_model* m)
 // ---- per-stream state records (stream_state.h / .cuh) ------------------------------------------------------------------
 // The handle's descriptor table, built once at creation.  A layout the record cannot describe (an internal mismatch) leaves
 // the handle working and only the stream-state calls refused, with the reason (nam_b200_model::state_error).
+// payload floats the conversion appends to a record (resample_in, resample_out, resample_phase), and its header word 3
+long rs_record_floats(const nam_b200_model* m)
+{
+  const auto& r = m->rs;
+  return r.active ? (long)m->spec.in_channels * r.H_up + (long)m->spec.out_channels * r.H_dn + 1 : 0;
+}
+uint32_t rs_ratio(const nam_b200_model* m)
+{
+  return m->rs.active ? ((uint32_t)m->rs.design.L << 16 | (uint32_t)m->rs.design.M) : 0u;
+}
+
 size_t record_bytes(const nam_b200_model* m)
 {
-  return (size_t)kStateHeaderBytes + 4 * (size_t)m->record_floats;
+  return (size_t)kStateHeaderBytes + 4 * (size_t)(m->record_floats + rs_record_floats(m));
 }
 
 void setup_state_records(nam_b200_model* m)
@@ -2096,6 +2335,122 @@ void import_records(nam_b200_model* m, const int32_t* streams, int n, const unsi
   CUDA_CHECK(cudaGetLastError());
   m->launches++;
   mark_written(m, streams, n);
+}
+
+// ---- the conversion's part of the per-stream state (a converting handle only) ------------------------------------------
+ResampleRecordParams rs_record_params(nam_b200_model* m, const int32_t* streams, int n, const uint32_t* phases, unsigned char* rec,
+                                      long stride, cudaStream_t st)
+{
+  std::vector<StreamRef> refs((size_t)n);
+  for (int i = 0; i < n; i++)
+    refs[(size_t)i] = StreamRef{streams[i], phases ? phases[i] : m->rs.phase[(size_t)streams[i]], 0, 0};
+  ResampleRecordParams p{};
+  p.hist = m->rs.d_hist;
+  p.hist_stride = m->rs.rs_stride;
+  p.in_channels = m->spec.in_channels;
+  p.out_channels = m->spec.out_channels;
+  p.H_up = m->rs.H_up;
+  p.H_dn = m->rs.H_dn;
+  p.refs = upload_refs(m, refs, st);
+  p.n = n;
+  p.rec = rec;
+  p.rec_stride = stride;
+  p.off = m->record_floats;
+  p.ratio = rs_ratio(m);
+  p.payload_floats = (uint64_t)(m->record_floats + rs_record_floats(m));
+  return p;
+}
+dim3 rs_record_grid(const nam_b200_model* m, int n)
+{
+  return dim3((unsigned)((rs_record_floats(m) - 1 + 255) / 256), (unsigned)std::min(n, 65535)); // (>= 1 item: H >= 1)
+}
+
+// after export_records into the same records: the conversion's segments and the header's ratio and payload count
+void rs_export(nam_b200_model* m, const int32_t* streams, int n, unsigned char* dst, long stride, cudaStream_t st)
+{
+  if (!m->rs.active)
+    return;
+  resample_pack_kernel<<<rs_record_grid(m, n), 256, 0, st>>>(rs_record_params(m, streams, n, nullptr, dst, stride, st));
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+}
+
+// the records' conversion segments into the streams; phases[i] = record i's resample_phase, checked by the caller
+void rs_import(nam_b200_model* m, const int32_t* streams, int n, const unsigned char* src, long stride, const uint32_t* phases,
+               cudaStream_t st)
+{
+  if (!m->rs.active)
+    return;
+  resample_unpack_kernel<<<rs_record_grid(m, n), 256, 0, st>>>(
+    rs_record_params(m, streams, n, phases, const_cast<unsigned char*>(src), stride, st));
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+  for (int i = 0; i < n; i++)
+    m->rs.phase[(size_t)streams[i]] = phases[i];
+}
+
+// record i's resample_phase (a float at the end of its payload) -> phases[i]; refused unless an integer in [0, M)
+int rs_record_phases(const nam_b200_model* m, const int32_t* streams, const float* values, int n, std::vector<uint32_t>* phases)
+{
+  phases->assign((size_t)n, 0u);
+  for (int i = 0; i < n; i++)
+  {
+    const float v = values[i];
+    if (!(v >= 0.0f && v < (float)m->rs.design.M && std::floor(v) == v))
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, "record " + std::to_string(i) + " (stream " + std::to_string(streams[i])
+                                                   + "): resample_phase " + std::to_string(v) + " is not an integer in [0, M="
+                                                   + std::to_string(m->rs.design.M) + ")");
+    (*phases)[(size_t)i] = (uint32_t)v;
+  }
+  return NAM_B200_OK;
+}
+
+// reset_streams / assign_streams: zero histories (row max_batch), h = 0
+void rs_zero(nam_b200_model* m, const int32_t* streams, int n, cudaStream_t st)
+{
+  if (!m->rs.active)
+    return;
+  std::vector<StreamRef> refs((size_t)2 * n);
+  for (int i = 0; i < n; i++)
+  {
+    refs[(size_t)i] = StreamRef{m->opts.max_batch, 0, 0, 0};
+    refs[(size_t)(n + i)] = StreamRef{streams[i], 0, 0, 0};
+    m->rs.phase[(size_t)streams[i]] = 0;
+  }
+  const StreamRef* d_refs = upload_refs(m, refs, st);
+  const long stride4 = m->rs.rs_stride / 4;
+  const dim3 grid((unsigned)((stride4 + kStateThreads - 1) / kStateThreads), (unsigned)std::min(n, 65535));
+  state_rows_kernel<<<grid, kStateThreads, 0, st>>>(reinterpret_cast<float4*>(m->rs.d_hist), reinterpret_cast<const float4*>(m->rs.d_hist),
+                                                     stride4, d_refs + n, d_refs, n);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches++;
+}
+
+// copy_streams: dst[i] takes src[i]'s conversion state, through scratch (a swap works)
+void rs_copy(nam_b200_model* m, const int32_t* src, const int32_t* dst, int n, cudaStream_t st)
+{
+  if (!m->rs.active)
+    return;
+  const long stride4 = m->rs.rs_stride / 4;
+  ensure_xfer(m, (size_t)n * m->rs.rs_stride * sizeof(float));
+  std::vector<StreamRef> refs((size_t)2 * n);
+  std::vector<uint32_t> ph((size_t)n);
+  for (int i = 0; i < n; i++)
+  {
+    refs[(size_t)i] = StreamRef{src[i], 0, 0, 0};
+    refs[(size_t)(n + i)] = StreamRef{dst[i], 0, 0, 0};
+    ph[(size_t)i] = m->rs.phase[(size_t)src[i]];
+  }
+  const StreamRef* d_refs = upload_refs(m, refs, st);
+  float4* scratch = reinterpret_cast<float4*>(m->d_xfer);
+  float4* hist = reinterpret_cast<float4*>(m->rs.d_hist);
+  const dim3 grid((unsigned)((stride4 + kStateThreads - 1) / kStateThreads), (unsigned)std::min(n, 65535));
+  state_rows_kernel<<<grid, kStateThreads, 0, st>>>(scratch, hist, stride4, nullptr, d_refs, n);
+  state_rows_kernel<<<grid, kStateThreads, 0, st>>>(hist, scratch, stride4, d_refs + n, nullptr, n);
+  CUDA_CHECK(cudaGetLastError());
+  m->launches += 2;
+  for (int i = 0; i < n; i++)
+    m->rs.phase[(size_t)dst[i]] = ph[(size_t)i];
 }
 
 // whole state rows: dst[dst_refs[i].stream or i] = src[src_refs[i].stream or i]
@@ -2554,9 +2909,9 @@ int check_process_args(nam_b200_model* m, const void* in, const void* out, int b
   if (batch < 1 || batch > m->opts.max_batch)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT,
                 "batch " + std::to_string(batch) + " outside [1, max_batch=" + std::to_string(m->opts.max_batch) + "]");
-  if (n_frames < 0 || n_frames > m->max_frames)
+  if (n_frames < 0 || n_frames > call_max_frames(m))
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "n_frames " + std::to_string(n_frames) + " exceeds max_frames "
-                                                 + std::to_string(m->max_frames) + " of the last reset");
+                                                 + std::to_string(call_max_frames(m)) + " of the last reset");
   return NAM_B200_OK;
 }
 
@@ -2591,7 +2946,7 @@ int process_planar(nam_b200_model* m, const T* const* input, T* const* output, i
       return NAM_B200_OK;
     const size_t ci = (size_t)m->spec.in_channels, co = (size_t)m->spec.out_channels, n = (size_t)n_frames;
     float* hin = m->h_pin;
-    float* hout = m->h_pin + (size_t)m->max_frames * std::max(ci, co);
+    float* hout = m->h_pin + (size_t)staging_frames(m) * std::max(ci, co);
     for (size_t c = 0; c < ci; c++)
       for (size_t i = 0; i < n; i++)
         hin[c * n + i] = (float)input[c][i];
@@ -2600,10 +2955,11 @@ int process_planar(nam_b200_model* m, const T* const* input, T* const* output, i
       float* din = m->h_pin_dev;
       float* dout = m->h_pin_dev + (hout - hin);
       m->flag_pending = false;
-      const bool doorbell = m->h_flag_dev != nullptr && n_frames <= 128 && !m->opts_timing_events;
+      // (a converting handle's last launch is the history update, not the model's: no doorbell)
+      const bool doorbell = m->h_flag_dev != nullptr && n_frames <= 128 && !m->opts_timing_events && !m->rs.active;
       if (!doorbell)
         CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-      run_device(m, din, dout, 1, n_frames, (long)(ci * n), (long)(co * n), m->stream);
+      run_call(m, din, dout, 1, n_frames, (long)(ci * n), (long)(co * n), m->stream);
       if (doorbell && m->flag_pending)
       {
         // the low-latency kernel served the call: wait for its doorbell (a word of host memory) -- no stream
@@ -2629,7 +2985,7 @@ int process_planar(nam_b200_model* m, const T* const* input, T* const* output, i
     {
       CUDA_CHECK(cudaMemcpyAsync(m->d_in, hin, ci * n * sizeof(float), cudaMemcpyHostToDevice, m->stream));
       CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-      run_device(m, m->d_in, m->d_out, 1, n_frames, (long)(ci * n), (long)(co * n), m->stream);
+      run_call(m, m->d_in, m->d_out, 1, n_frames, (long)(ci * n), (long)(co * n), m->stream);
       CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
       CUDA_CHECK(cudaMemcpyAsync(hout, m->d_out, co * n * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
     }
@@ -2672,11 +3028,33 @@ int check_stream_list(const nam_b200_model* m, const int32_t* idx, int n, const 
   return NAM_B200_OK;
 }
 
-int check_records(const nam_b200_model* m, const void* buf, int n, int64_t stride, bool device)
+// a record's header word 3 must hold the handle's conversion ratio (0 when it converts nothing)
+int check_record_ratio(const nam_b200_model* m, const StateRecordHeader& h, const std::string& at)
+{
+  if (h.reserved == rs_ratio(m))
+    return NAM_B200_OK;
+  auto ratio = [](uint32_t r) { return r ? std::to_string(r >> 16) + "/" + std::to_string(r & 0xffffu) : std::string("none"); };
+  return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "resample ratio (header word 3) " + ratio(h.reserved) + ", this handle's is "
+                                               + ratio(rs_ratio(m)) + " (model / host rate, as of its last reset)");
+}
+
+// `incoming`: records to import -- a stride too small for this handle's record is first checked for a conversion ratio
+// that differs from the handle's (a record of another rate pair has another size), so that the refusal names the cause
+int check_records(const nam_b200_model* m, const void* buf, int n, int64_t stride, bool device, bool incoming = false)
 {
   if (n > 0 && !buf)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null record buffer");
   const size_t rb = record_bytes(m);
+  if (stride < (int64_t)rb && incoming && n > 0 && stride >= kStateHeaderBytes)
+  {
+    StateRecordHeader h;
+    if (device)
+      CUDA_CHECK(cudaMemcpy(&h, buf, sizeof h, cudaMemcpyDeviceToHost));
+    else
+      std::memcpy(&h, buf, sizeof h);
+    if (std::memcmp(h.magic, "NAMS", 4) == 0 && check_record_ratio(m, h, "record 0: ") != NAM_B200_OK)
+      return NAM_B200_ERR_INVALID_ARGUMENT;
+  }
   if (stride < (int64_t)rb)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "record_stride " + std::to_string(stride) + " is smaller than the record ("
                                                  + std::to_string(rb) + " bytes)");
@@ -2706,9 +3084,12 @@ int check_record_header(const nam_b200_model* m, const unsigned char* rec, int i
   if (h.architecture != want.architecture)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "architecture " + std::to_string(h.architecture) + ", the model's is "
                                                  + std::to_string(want.architecture));
-  if (h.payload_floats != want.payload_floats)
+  if (check_record_ratio(m, h, at) != NAM_B200_OK)
+    return NAM_B200_ERR_INVALID_ARGUMENT;
+  const uint64_t payload = want.payload_floats + (uint64_t)rs_record_floats(m);
+  if (h.payload_floats != payload)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, at + "payload float count " + std::to_string(h.payload_floats)
-                                                 + ", the model's record holds " + std::to_string(want.payload_floats));
+                                                 + ", the model's record holds " + std::to_string(payload));
   if (m->is_bank)
   {
     for (int k = 0; k < m->bank_size; k++)
@@ -2741,7 +3122,7 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
   const size_t row = (size_t)n_frames * sizeof(float);
   const bool padded = counts != nullptr && std::any_of(counts, counts + n, [&](int32_t c) { return c < n_frames; });
   const int chunk = wavenet_chunk_streams(m);
-  if (chunk > 0 && n >= 2 * chunk && (size_t)n * row >= ((size_t)8 << 20))
+  if (chunk > 0 && n >= 2 * chunk && (size_t)n * row >= ((size_t)8 << 20) && !m->rs.active)
   {
     const int n_chunks = (n + chunk - 1) / chunk;
     if (!m->copy_in)
@@ -2794,7 +3175,7 @@ void process_host(nam_b200_model* m, const int32_t* streams, int n, const float*
   if (padded)
     CUDA_CHECK(cudaMemsetAsync(m->d_out, 0, (size_t)n * co * row, m->stream));
   CUDA_CHECK(cudaEventRecord(m->ev0, m->stream));
-  run_device(m, m->d_in, m->d_out, n, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream, streams, counts);
+  run_call(m, m->d_in, m->d_out, n, n_frames, (long)(ci * n_frames), (long)(co * n_frames), m->stream, streams, counts);
   CUDA_CHECK(cudaEventRecord(m->ev1, m->stream));
   CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)out_stride * sizeof(float), m->d_out, co * row, co * row, (size_t)n,
                                cudaMemcpyDeviceToHost, m->stream));
@@ -2812,9 +3193,9 @@ int check_process_streams_args(const nam_b200_model* m, const char* fn, const in
   if (n < 0 || n > m->opts.max_batch)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT,
                 f + ": n = " + std::to_string(n) + " outside [0, max_batch=" + std::to_string(m->opts.max_batch) + "]");
-  if (n_frames < 0 || n_frames > m->max_frames)
+  if (n_frames < 0 || n_frames > call_max_frames(m))
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": n_frames " + std::to_string(n_frames) + " outside [0, max_frames="
-                                                 + std::to_string(m->max_frames) + "] of the last reset");
+                                                 + std::to_string(call_max_frames(m)) + "] of the last reset");
   if (n == 0 || n_frames == 0)
     return NAM_B200_OK;
   if (!in || !out)
@@ -2847,9 +3228,9 @@ int check_ragged_args(const nam_b200_model* m, const char* fn, const int32_t* st
       return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": null n_frames");
     for (int i = 0; i < n; i++)
     {
-      if (n_frames[i] < 0 || n_frames[i] > m->max_frames)
+      if (n_frames[i] < 0 || n_frames[i] > call_max_frames(m))
         return fail(NAM_B200_ERR_INVALID_ARGUMENT, f + ": n_frames[" + std::to_string(i) + "] = " + std::to_string(n_frames[i])
-                                                     + " outside [0, max_frames=" + std::to_string(m->max_frames)
+                                                     + " outside [0, max_frames=" + std::to_string(call_max_frames(m))
                                                      + "] of the last reset");
       *n_max = std::max(*n_max, (int)n_frames[i]);
     }
@@ -3637,7 +4018,7 @@ static int fill_info(const nam_b200_model* m, const ModelSpec& spec, nam_b200_in
   r.out_channels = spec.out_channels;
   r.prewarm_samples = spec.prewarm_samples;
   r.max_batch = m->opts.max_batch;
-  r.max_frames = m->max_frames;
+  r.max_frames = call_max_frames(m);
   r.has_loudness = spec.loudness.has_value();
   r.has_input_level = spec.input_level.has_value();
   r.has_output_level = spec.output_level.has_value();
@@ -3651,6 +4032,9 @@ static int fill_info(const nam_b200_model* m, const ModelSpec& spec, nam_b200_in
   r.kernel_variant = m->variant;
   r.jit_state = m->spec_state;
   r.jit_lat_state = m->lat_state;
+  r.resample_up = m->rs.active ? m->rs.design.L : 1;
+  r.resample_down = m->rs.active ? m->rs.design.M : 1;
+  r.resample_latency_frames = m->rs.active ? (int32_t)std::lround(m->rs.design.latency_frames) : 0;
   const size_t n = std::min<size_t>(sizeof(r), (size_t)std::max(info->struct_size, 0));
   const int32_t user_size = info->struct_size;
   std::memcpy(info, &r, n);
@@ -3668,7 +4052,8 @@ int nam_b200_get_info(const nam_b200_model* m, nam_b200_info* info)
 
 int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
 {
-  // like the reference, the external rate is recorded but does not change the arithmetic
+  // like the reference, the external rate is recorded but does not change the model's arithmetic (options.resample
+  // converts to the model's rate around it)
   if (m && m->active_sub >= 0)
   {
     // ContainerModel::Reset (container.cpp:73-86): remember the settings, reset only the active sub-model
@@ -3682,10 +4067,15 @@ int nam_b200_reset(nam_b200_model* m, double sample_rate, int max_frames)
   return guarded(m, [&]() -> int {
     if (max_frames < 1)
       return fail(NAM_B200_ERR_INVALID_ARGUMENT, "max_frames must be >= 1");
-    m->max_frames = max_frames;
+    ResamplerDesign rd;
+    bool convert = false;
+    const std::string refusal = resampler_for(m, sample_rate, &rd, &convert);
+    if (!refusal.empty())
+      return fail(NAM_B200_ERR_INVALID_ARGUMENT, refusal);
+    setup_resampler(m, convert, rd, max_frames); // (m->max_frames: the model's maxBufferSize)
     const size_t ch = (size_t)std::max(m->spec.in_channels, m->spec.out_channels);
-    ensure_staging(m, (size_t)m->opts.max_batch * max_frames * ch);
-    ensure_pinned(m, (size_t)2 * max_frames * ch);
+    ensure_staging(m, (size_t)m->opts.max_batch * staging_frames(m) * ch);
+    ensure_pinned(m, (size_t)2 * staging_frames(m) * ch);
     ensure_hist(m);
     setup_lat_kernel(m);
     if (m->spec.arch == Arch::WaveNet && !m->h_flag && m->opts.max_batch <= m->sm_count && max_frames <= 128
@@ -3759,6 +4149,7 @@ int nam_b200_reset_streams(nam_b200_model* m, const int32_t* streams, int n, int
       bank_fan_out(m, streams, n, m->stream); // each stream's own model's fresh row
     else
       import_records(m, streams, n, m->d_fresh, 0, m->stream); // (fresh or not: Reset forgets the past)
+    rs_zero(m, streams, n, m->stream);
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return NAM_B200_OK;
   });
@@ -3808,6 +4199,7 @@ int nam_b200_copy_streams(nam_b200_model* m, const int32_t* src, const int32_t* 
       m->stream_flips[(size_t)dst[i]] = flips[(size_t)i];
       m->stream_model[(size_t)dst[i]] = model[(size_t)i];
     }
+    rs_copy(m, src, dst, n, m->stream);
     m->streams_identical = false;
     recount_phase(m);
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -3833,6 +4225,7 @@ int nam_b200_export_streams(nam_b200_model* m, const int32_t* streams, int n, vo
     {
       const int k = std::min(group, n - i0);
       export_records(m, streams + i0, k, m->d_xfer, (long)rb, m->stream);
+      rs_export(m, streams + i0, k, m->d_xfer, (long)rb, m->stream);
       CUDA_CHECK(cudaMemcpy2DAsync(static_cast<unsigned char*>(dst) + (size_t)i0 * record_stride, (size_t)record_stride, m->d_xfer,
                                    rb, rb, (size_t)k, cudaMemcpyDeviceToHost, m->stream));
       CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -3849,10 +4242,19 @@ int nam_b200_import_streams(nam_b200_model* m, const int32_t* streams, int n, co
     if (rc == NAM_B200_OK)
       rc = check_stream_list(m, streams, n, "streams", true);
     if (rc == NAM_B200_OK)
-      rc = check_records(m, src, n, record_stride, false);
+      rc = check_records(m, src, n, record_stride, false, true);
     std::vector<int> model((size_t)std::max(n, 0));
     for (int i = 0; i < n && rc == NAM_B200_OK; i++)
       rc = check_record_header(m, static_cast<const unsigned char*>(src) + (size_t)i * record_stride, i, streams[i], &model[(size_t)i]);
+    std::vector<uint32_t> phases;
+    if (rc == NAM_B200_OK && m->rs.active)
+    {
+      std::vector<float> v((size_t)n);
+      const size_t at = kStateHeaderBytes + 4 * (size_t)(m->record_floats + rs_record_floats(m) - 1);
+      for (int i = 0; i < n; i++)
+        std::memcpy(&v[(size_t)i], static_cast<const unsigned char*>(src) + (size_t)i * record_stride + at, 4);
+      rc = rs_record_phases(m, streams, v.data(), n, &phases);
+    }
     if (rc != NAM_B200_OK || n == 0)
       return rc;
     for (int i = 0; i < n; i++) // (a bank: the stream runs the record's model from now on)
@@ -3866,6 +4268,7 @@ int nam_b200_import_streams(nam_b200_model* m, const int32_t* streams, int n, co
       CUDA_CHECK(cudaMemcpy2DAsync(m->d_xfer, rb, static_cast<const unsigned char*>(src) + (size_t)i0 * record_stride,
                                    (size_t)record_stride, rb, (size_t)k, cudaMemcpyHostToDevice, m->stream));
       import_records(m, streams + i0, k, m->d_xfer, (long)rb, m->stream);
+      rs_import(m, streams + i0, k, m->d_xfer, (long)rb, phases.data() + i0, m->stream);
       CUDA_CHECK(cudaStreamSynchronize(m->stream));
     }
     return NAM_B200_OK;
@@ -3886,6 +4289,7 @@ int nam_b200_export_streams_device(nam_b200_model* m, const int32_t* streams, in
       return rc;
     const cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
     export_records(m, streams, n, static_cast<unsigned char*>(dst_device), (long)record_stride, st);
+    rs_export(m, streams, n, static_cast<unsigned char*>(dst_device), (long)record_stride, st);
     return NAM_B200_OK;
   });
 }
@@ -3899,7 +4303,7 @@ int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, in
     if (rc == NAM_B200_OK)
       rc = check_stream_list(m, streams, n, "streams", true);
     if (rc == NAM_B200_OK)
-      rc = check_records(m, src_device, n, record_stride, true);
+      rc = check_records(m, src_device, n, record_stride, true, true);
     if (rc != NAM_B200_OK || n == 0)
       return rc;
     const cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
@@ -3907,6 +4311,12 @@ int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, in
     std::vector<unsigned char> headers((size_t)n * kStateHeaderBytes);
     CUDA_CHECK(cudaMemcpy2DAsync(headers.data(), kStateHeaderBytes, src_device, (size_t)record_stride, kStateHeaderBytes, (size_t)n,
                                  cudaMemcpyDeviceToHost, st));
+    std::vector<float> phase_values((size_t)n); // (a converting handle: each record's resample_phase, the payload's last float)
+    if (m->rs.active)
+      CUDA_CHECK(cudaMemcpy2DAsync(phase_values.data(), 4,
+                                   static_cast<const unsigned char*>(src_device) + kStateHeaderBytes
+                                     + 4 * (size_t)(m->record_floats + rs_record_floats(m) - 1),
+                                   (size_t)record_stride, 4, (size_t)n, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     std::vector<int> model((size_t)n);
     for (int i = 0; i < n; i++)
@@ -3915,11 +4325,30 @@ int nam_b200_import_streams_device(nam_b200_model* m, const int32_t* streams, in
       if (rc != NAM_B200_OK)
         return rc;
     }
+    std::vector<uint32_t> phases;
+    if (m->rs.active && (rc = rs_record_phases(m, streams, phase_values.data(), n, &phases)) != NAM_B200_OK)
+      return rc;
     for (int i = 0; i < n; i++)
       m->stream_model[(size_t)streams[i]] = model[(size_t)i];
     import_records(m, streams, n, static_cast<const unsigned char*>(src_device), (long)record_stride, st);
+    rs_import(m, streams, n, static_cast<const unsigned char*>(src_device), (long)record_stride, phases.data(), st);
     return NAM_B200_OK;
   });
+}
+
+int nam_b200_resampler_json(double host_rate, double model_rate, char* out, int64_t capacity)
+{
+  if (!out || capacity < 1)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "null or empty output buffer");
+  ResamplerDesign d;
+  std::string why;
+  if (!design_resampler(host_rate, model_rate, &d, &why))
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, why);
+  const std::string js = resampler_json(d);
+  if ((int64_t)js.size() >= capacity)
+    return fail(NAM_B200_ERR_INVALID_ARGUMENT, "output buffer too small: " + std::to_string(js.size() + 1) + " bytes needed");
+  std::memcpy(out, js.c_str(), js.size() + 1);
+  return NAM_B200_OK;
 }
 
 int nam_b200_state_layout_json(const char* nam_json_text, char* out, int64_t capacity)
@@ -4197,6 +4626,7 @@ int nam_b200_assign_streams(nam_b200_model* m, const int32_t* streams, int n, co
     for (int i = 0; i < n; i++)
       m->stream_model[(size_t)streams[i]] = models[i];
     bank_fan_out(m, streams, n, m->stream);
+    rs_zero(m, streams, n, m->stream);
     CUDA_CHECK(cudaStreamSynchronize(m->stream));
     return NAM_B200_OK;
   });
@@ -4240,7 +4670,7 @@ int nam_b200_process_f32_device(nam_b200_model* m, const float* in_device, float
       return NAM_B200_OK;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
     CUDA_CHECK(cudaEventRecord(m->ev0, st));
-    run_device(m, in_device, out_device, batch, n_frames, (long)in_stride, (long)out_stride, st);
+    run_call(m, in_device, out_device, batch, n_frames, (long)in_stride, (long)out_stride, st);
     CUDA_CHECK(cudaEventRecord(m->ev1, st));
     m->timing_valid = true;
     return NAM_B200_OK;
@@ -4290,7 +4720,7 @@ int nam_b200_process_streams_f32_device(nam_b200_model* m, const int32_t* stream
       return rc;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
     CUDA_CHECK(cudaEventRecord(m->ev0, st));
-    run_device(m, in_device, out_device, n, n_frames, (long)in_stride, (long)out_stride, st, streams);
+    run_call(m, in_device, out_device, n, n_frames, (long)in_stride, (long)out_stride, st, streams);
     CUDA_CHECK(cudaEventRecord(m->ev1, st));
     m->timing_valid = true;
     return NAM_B200_OK;
@@ -4325,7 +4755,7 @@ int nam_b200_process_streams_ragged_f32_device(nam_b200_model* m, const int32_t*
       return rc;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
     CUDA_CHECK(cudaEventRecord(m->ev0, st));
-    run_device(m, in_device, out_device, n, n_max, (long)in_stride, (long)out_stride, st, streams, n_frames);
+    run_call(m, in_device, out_device, n, n_max, (long)in_stride, (long)out_stride, st, streams, n_frames);
     CUDA_CHECK(cudaEventRecord(m->ev1, st));
     m->timing_valid = true;
     return NAM_B200_OK;
@@ -4419,6 +4849,9 @@ int multi_create(const char* text_or_path, bool is_file, const nam_b200_options*
   o.struct_size = sizeof o;
   if (o.max_batch < n_devices)
     return fail(NAM_B200_ERR_INVALID_ARGUMENT, "max_batch is smaller than the number of devices");
+  if (o.resample != 0)
+    return fail(NAM_B200_ERR_UNSUPPORTED, "resample = " + std::to_string(o.resample)
+                                            + ": multi-GPU handles do not convert sample rates (use one handle per GPU)");
   std::unique_ptr<nam_b200_multi> mm(new nam_b200_multi());
   int s0 = 0;
   for (int i = 0; i < n_devices; i++)

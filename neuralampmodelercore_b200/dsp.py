@@ -180,6 +180,18 @@ class DSP:
         self._refresh_info()
         return int(self._info.jit_lat_state)
 
+    @property
+    def resample_ratio(self) -> tuple:
+        """(L, M): the conversion of the last Reset, model rate / host rate = L / M; (1, 1) when none."""
+        self._refresh_info()
+        return int(self._info.resample_up), int(self._info.resample_down)
+
+    @property
+    def resample_latency(self) -> int:
+        """Group delay of the conversion in host frames, rounded (resampler()['latency_frames'] exactly); 0 when none."""
+        self._refresh_info()
+        return int(self._info.resample_latency_frames)
+
     def jit_note(self) -> str:
         buf = C.create_string_buffer(4096)
         self._lib.nam_b200_jit_note(self._h, buf, len(buf))
@@ -515,7 +527,7 @@ class DSP:
 
 
 def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: Optional[bool], ctas_per_sm: int,
-             kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0, capacity: int = 0):
+             kernel_geometry: int = 0, tile_mode: int = 0, jit: int = 0, capacity: int = 0, resample: bool = False):
     o = _capi.Options()
     lib.nam_b200_default_options(C.byref(o))
     o.device = int(device)
@@ -527,12 +539,13 @@ def _options(lib, batch: int, device: int, prewarm: Optional[bool], fast_tanh: O
     o.tile_mode = int(tile_mode)
     o.jit = int(jit)
     o.bank_capacity = int(capacity)
+    o.resample = int(bool(resample))
     return o
 
 
 def get_dsp(config, batch: int = 1, device: int = -1, prewarm: Optional[bool] = None,
             fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
-            tile_mode: int = 0, jit: int = 0) -> DSP:
+            tile_mode: int = 0, jit: int = 0, resample: bool = False) -> DSP:
     """nam::get_dsp: `config` is a path to a .nam file, a dict (parsed .nam) or a JSON string.
 
     batch      number of independent streams the handle carries (the reference: one DSP object each)
@@ -540,11 +553,14 @@ def get_dsp(config, batch: int = 1, device: int = -1, prewarm: Optional[bool] = 
     fast_tanh  None = use the process-wide switch (enable_fast_tanh()), like the reference
     kernel_geometry / tile_mode / ctas_per_sm   tuning knobs, see nam_b200_options (include/nam_b200.h)
     jit         model-specialised kernel (NVRTC at load): 0 = default (on for batch >= 256), 1 = required, 2 = off
+    resample    True = Reset(sampleRate) at a rate other than the model's converts every stream to the model's rate and
+                back on the device (resampler(); DSP.resample_ratio, DSP.resample_latency); False = the reference's
+                behaviour: the rate is recorded and ignored
     """
     import json
 
     lib = _capi.load()
-    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit)
+    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit, resample=resample)
     h = C.c_void_p()
     if isinstance(config, (str, os.PathLike)) and not (isinstance(config, str) and config.lstrip().startswith("{")):
         rc = lib.nam_b200_create_from_file(str(Path(config)).encode(), C.byref(o), C.byref(h))
@@ -576,7 +592,7 @@ def _text_array(texts: list):
 
 def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bool] = None,
                  fast_tanh: Optional[bool] = None, ctas_per_sm: int = 0, kernel_geometry: int = 0,
-                 tile_mode: int = 0, jit: int = 0, capacity: int = 0) -> DSP:
+                 tile_mode: int = 0, jit: int = 0, capacity: int = 0, resample: bool = False) -> DSP:
     """A model bank: one handle of `batch` streams over the K documents in `configs` (paths, dicts or JSON texts), which
     must share one shape (bank_check): WaveNets of the fused kernel family, WaveNets of the general kernel (A2-style,
     condition_dsp, multi-channel), ConvNets, or LSTMs.  Every stream starts bound to model
@@ -588,9 +604,10 @@ def get_dsp_bank(configs, batch: int = 1, device: int = -1, prewarm: Optional[bo
     run the precompiled kernels under 0 / 3; a ConvNet bank takes it as an ordinary ConvNet handle.  kernel_geometry = 4
     is refused for fused-family and LSTM banks; on a general bank it selects the precompiled general kernel, and a
     ConvNet bank ignores it.  capacity: the models the bank can hold (0 = len(configs)); room for DSP.add_models is
-    reserved at creation.  A bank of one document and capacity 0 or 1 is get_dsp."""
+    reserved at creation.  A bank of one document and capacity 0 or 1 is get_dsp.  resample: as get_dsp's; the bank's
+    models share one expected rate, hence one conversion."""
     lib = _capi.load()
-    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit, capacity)
+    o = _options(lib, batch, device, prewarm, fast_tanh, ctas_per_sm, kernel_geometry, tile_mode, jit, capacity, resample)
     arr, _keep = _text_array(_documents(configs))
     h = C.c_void_p()
     rc = lib.nam_b200_create_bank_from_json(arr, len(_keep), C.byref(o), C.byref(h))
@@ -669,6 +686,23 @@ def inspect(config, fast_tanh: Optional[bool] = None) -> dict:
     if rc != 0:
         _raise(rc, lib)
     return json.loads(buf.value.decode())
+
+
+def resampler(host_rate: float, model_rate: float) -> dict:
+    """Host-only: the sample-rate conversion between these rates (get_dsp(resample=True)): L, M (model / host = L / M),
+    n_taps, taps_per_output_up / _down, latency_frames (host frames) and the float32 taps g_up, g_dn as numpy arrays.
+    Pairs Reset would refuse raise ValueError naming both rates.  Needs no GPU."""
+    import json
+
+    lib = _capi.load()
+    buf = C.create_string_buffer(1 << 20)
+    rc = lib.nam_b200_resampler_json(float(host_rate), float(model_rate), buf, len(buf))
+    if rc != 0:
+        _raise(rc, lib)
+    d = json.loads(buf.value.decode())
+    d["g_up"] = np.asarray(d["g_up"], dtype=np.float32)
+    d["g_dn"] = np.asarray(d["g_dn"], dtype=np.float32)
+    return d
 
 
 def state_layout(config) -> dict:
